@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- RNN-T loss+grad utterances/sec (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- RNN-T loss+grad utterances/sec (BASELINE.json metric) on N H100s of one node.
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
   python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path on the host cores
@@ -11,10 +11,15 @@ batch; --scaling strong = BASELINE C4 literally (ONE global batch of B utterance
 N=8).  An N>1 weak run also measures the strong point and reports it under "strong".  The only collective is ONE
 packed all-reduce of [loss_sum | dW | db] per step.
 
-Printed JSON (one line, rank 0): see the task contract -- value (inputs resident in HBM), e2e (host
-buffers through the public torch API, H2D/D2H inside the timed region), roofline of the dominant
-kernel (CUDA events on the launching stream, attribution pass outside the timed region),
-cpu_baseline (reference library + torch-CPU joint on the host cores), clocks, gpu_launches.
+Printed JSON (one line, rank 0): value (inputs resident in HBM), e2e (host buffers through the public
+torch API, H2D/D2H inside the timed region), roofline of the dominant kernel (CUDA events on the
+launching stream, attribution pass outside the timed region), cpu_baseline (reference library +
+torch-CPU joint on the host cores), clocks, gpu_launches.
+
+--dump-outputs DIR writes what the last timed step returned to its caller -- the mean loss, the
+per-utterance costs and the gradients d_enc, d_pred, dW, db -- as DIR/<name>.npy (float32; an array
+beyond its share of 64 MB is replaced by a fixed, seeded sample of its elements).  The inputs are
+seeded, so two builds of the library can be compared output for output.
 """
 import argparse
 import json
@@ -40,36 +45,30 @@ METRIC = "rnnt_loss_grad_utterances_per_sec"
 
 
 def peaks():
+    """H100 SXM data-sheet peaks (700 W card: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16), unless MEASURED_PEAKS.json
+    holds measured ones.  A power-limited card reaches less; `clocks` in the result line shows what it ran at."""
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
-def csrc_sha16():
-    """Hash of the CUDA sources: an ncu capture is only quoted next to a number when it was taken from THIS source."""
-    import glob
-    import hashlib
-    h = hashlib.sha256()
-    for f in sorted(glob.glob(os.path.join(ROOT, "rnnt_speech_recognition_b200", "csrc", "*.cu*"))):
-        h.update(open(f, "rb").read())
-    return h.hexdigest()[:16]
+DUMP_BUDGET = 64 << 20
 
 
-def measured_traffic():
-    """profiles/rNN/traffic.json = {"csrc_sha16": ..., "kernels": {name: dram bytes per launch}, "step": bytes} written by
-    tools/ncu_summary.py from an `ncu --set full` capture.  Returned only if it was captured from the current sources
-    (otherwise the figure would silently go stale the moment a kernel changes)."""
-    import glob
-    for f in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*", "traffic.json")), reverse=True):
-        try:
-            t = json.load(open(f))
-            if t.get("csrc_sha16") == csrc_sha16():
-                t["file"] = os.path.relpath(f, ROOT)
-                return t
-        except Exception:
-            pass
-    return None
+def dump_outputs(outdir, arrays):
+    """arrays: {name: tensor} -> outdir/<name>.npy in float32.  Arrays are sampled (a fixed seeded choice of flat indices,
+    sorted) down to an equal share of DUMP_BUDGET when the whole set would exceed it."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    host = {k: v.detach().float().cpu().numpy().reshape(-1) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    share = DUMP_BUDGET // max(1, len(host)) // 4
+    for i, (k, a) in enumerate(sorted(host.items())):
+        if total > DUMP_BUDGET and a.size > share:
+            idx = np.sort(np.random.default_rng(1234 + i).choice(a.size, share, replace=False))
+            a = a[idx]
+        np.save(os.path.join(outdir, k + ".npy"), np.ascontiguousarray(a, np.float32))
 
 
 def synth(cfg, seed, device, pin=False):
@@ -95,7 +94,7 @@ def synth(cfg, seed, device, pin=False):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -229,13 +228,13 @@ def workload_config(cfg, n_gpus, name, scaling="weak"):
                            "GLOBAL batch sharded over the GPUs" if strong else "per GPU",
                            " (ragged T_b in [100,T], U_b in [10,U])" if cfg.get("ragged") else ""),
             "global_batch": cfg["B"] * (1 if strong else n_gpus), "parallelism": "dp%d" % n_gpus, "precision": cfg["precision"],
-            "l2": "256 MiB scratch write between timed steps; per-step working set (>4 GB) exceeds the 126 MB L2"}
+            "l2": "256 MiB scratch write between timed steps; per-step working set (>4 GB) exceeds the 50 MB L2"}
 
 
 def op_path_block(pk):
     """Materialised-logits entry (compute_rnnt_loss, the warp-transducer-compatible C ABI) on this GPU: ms per call,
     achieved GB/s on SURVEY 8(d)'s algorithmic bytes 3*N*V*4 + 24*N against the measured HBM peak, and the reference's
-    own SIMT kernels (oracle/_ref/libwarprnnt_gpu.so, compiled unmodified for sm_100) on the same inputs."""
+    own SIMT kernels (oracle/_ref/libwarprnnt_gpu.so, compiled unmodified for sm_90) on the same inputs."""
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     try:
         import bench_op
@@ -260,6 +259,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-op-path", action="store_true")
     ap.add_argument("--cpu-budget", type=float, default=20.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (loss, costs, d_enc, d_pred, dW, db) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     cfg = WORKLOADS[args.workload]
@@ -314,13 +315,14 @@ def main():
         loss_sum = costs.sum()
         (loss_sum / mode["gB"]).backward()                           # run_rnnt.py:278
         ls, dW, db = D.allreduce_loss_and_weight_grads(loss_sum.detach(), params[0].grad, params[1].grad)
-        return ls / mode["gB"], enc.grad, pred.grad, dW, db
+        return ls / mode["gB"], enc.grad, pred.grad, dW, db, costs.detach()
 
     cur = {"d": d}
 
     def resident_step():
         x = cur["d"]
-        return step(x["enc"].detach(), x["pred"].detach(), x["labels"], x["il"], x["ll"])
+        cur["last"] = step(x["enc"].detach(), x["pred"].detach(), x["labels"], x["il"], x["ll"])
+        return cur["last"]
 
     # e2e: every step copies ITS inputs from pinned host memory and reads its loss back.  The copy of step i+1 is
     # issued on a copy stream while step i computes (what a prefetching input pipeline does); the compute stream
@@ -373,6 +375,8 @@ def main():
     l0 = _lib.launch_count()
     ms = timed(resident_step, args.steps)
     launches = _lib.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(zip(("loss", "d_enc", "d_pred", "dW", "db", "costs"), cur["last"])))
     for _ in range(2):
         e2e_step()
     ms_e2e = timed(e2e_step, args.steps)
@@ -414,17 +418,15 @@ def main():
     if rank == 0:
         pk, pk_src = peaks()
         N = int((d["il"].long() * (d["ll"].long() + 1)).sum().item())      # valid lattice cells of this rank (== B*T*U when not ragged)
-        traffic = measured_traffic()
         if cfg["precision"] == "bf16":
             flops = 2.0 * N * H * V
-            dom = next((k for k in kernels if k.endswith("<fwd>") or k.endswith("<fwd+keep>")), "joint_tc3_kernel<fwd+keep>")
+            dom = next((k for k in kernels if k.endswith("<fwd>") or k.endswith("<fwd+keep>")), "joint_fwd_kernel<fwd+keep>")
             t_dom = kernels.get(dom)
             ach = flops / (t_dom * 1e-3) / 1e12 if t_dom else None
-            peak = pk["bf16_tflops_sustained"]
+            peak = pk["bf16_tflops"]
             roof = {"kernel": dom, "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
                     "frac": (ach / peak) if ach else None,
-                    "traffic": (traffic or {}).get("kernels", {}).get(dom),
-                    "peak_source": "%s bf16 sustained (kernel timed inside the step)" % pk_src,
+                    "peak_source": "%s dense bf16 (kernel timed inside the step)" % pk_src,
                     "algorithmic_flops_per_launch": flops, "launch_ms": t_dom,
                     "step": {"algorithmic_flops": 6.0 * N * H * V,
                              "achieved": 6.0 * N * H * V / (ms / args.steps * 1e-3) / 1e12,
@@ -435,8 +437,7 @@ def main():
             byts = 24.0 * N
             ach = byts / (t_dom * 1e-3) / 1e9 if t_dom else None
             roof = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                    "frac": (ach / pk["hbm_gbs"]) if ach else None,
-                    "traffic": (traffic or {}).get("kernels", {}).get(dom), "peak_source": pk_src,
+                    "frac": (ach / pk["hbm_gbs"]) if ach else None, "peak_source": pk_src,
                     "algorithmic_bytes_per_launch": byts, "launch_ms": t_dom}
         h2d = sum(host[k].numel() * host[k].element_size() for k in ("enc", "pred", "labels", "il", "ll"))
         out = {
@@ -457,8 +458,6 @@ def main():
                                            "ms_per_step": ms_nomat / args.steps,
                                            "note": "keep_activations=0: nothing of size O(N*V) survives the forward call; "
                                                    "`value` is the default mode (forward keeps 2 B per logit for the backward)"}
-        out["dram_bytes_per_step"] = ({"value": traffic.get("step"), "source": traffic["file"] + " (ncu --set full of this "
-                                       "source tree, csrc_sha16 %s)" % traffic["csrc_sha16"]} if traffic else None)
         if strong:
             out["strong"] = strong
         if world == 1 and not args.no_op_path and args.workload == "c3":

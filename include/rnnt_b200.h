@@ -1,5 +1,5 @@
 /** \file rnnt_b200.h
- *  C ABI of librnnt_b200.so -- the B200-native (sm_100a) RNN-T loss hot path.
+ *  C ABI of librnnt_b200.so -- the H100-native (sm_90a) RNN-T loss hot path.
  *
  *  Part 1 is a drop-in for the warp-transducer C interface the reference application binds
  *  (reference: warp-transducer/include/rnnt.h:16-143, implemented in
@@ -132,7 +132,7 @@ rnntStatus_t rnntb200_loss_device(const float* activations, float* gradients, co
 
 typedef enum {
     RNNTB200_FP32_EXACT = 0, /**< fp32 CUDA-core arithmetic; parity gate rtol 1e-4 (BASELINE C1/C2) */
-    RNNTB200_BF16_TC = 1     /**< 16-bit operands on tcgen05 tensor cores, fp32 accumulate (BASELINE C3-C5): the forward
+    RNNTB200_BF16_TC = 1     /**< 16-bit operands on wgmma tensor cores, fp32 accumulate (BASELINE C3-C5): the forward
                                   projection runs on fp16 z / W (11-bit significands), the two gradient GEMMs on bf16 */
 } rnntb200Precision;
 
@@ -226,7 +226,7 @@ unsigned long long rnntb200_launch_count();
 void rnntb200_set_timing(int on);
 int rnntb200_get_timing(int index, const char** name, float* ms);
 
-/** Build info string: "rnnt_b200 <version> sm_100a tcgen05=<0|1>". */
+/** Build info string: "rnnt_b200 <version> sm_90a wgmma=<0|1>". */
 const char* rnntb200_build_info();
 
 #ifdef __cplusplus

@@ -4,8 +4,8 @@ Two back-ends, both CPU-only:
 
 * ``liboracle.so``  -- the C restatement in ``oracle/rnnt_oracle.c`` (each C function cites
   the reference file:line it follows).
-* ``oracle/_ref/libwarprnnt.so`` -- the UNMODIFIED reference library compiled from
-  ``/root/reference/warp-transducer`` by ``oracle/Makefile`` (when present).  Its C ABI is
+* ``oracle/_ref/libwarprnnt.so`` -- the UNMODIFIED reference library compiled by ``oracle/Makefile`` from the
+  warp-transducer checkout that ``WARP_TRANSDUCER_DIR`` names (when it is set).  Its C ABI is
   ``warp-transducer/include/rnnt.h:16-143``; ``rnntOptions`` is passed by value.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / reference arm may
@@ -23,14 +23,18 @@ _REF = None
 
 
 def build(force=False):
-    """Compile liboracle.so (and oracle/_ref when /root/reference is present)."""
+    """Compile liboracle.so (and oracle/_ref when WARP_TRANSDUCER_DIR names the reference sources)."""
     so = os.path.join(_HERE, "liboracle.so")
     src = [os.path.join(_HERE, f) for f in ("rnnt_oracle.c", "rnnt_oracle_impl.inc")]
     stale = (not os.path.exists(so)) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in src)
-    if force or stale or (os.path.isdir("/root/reference/warp-transducer/src")
-                          and not os.path.exists(os.path.join(_HERE, "_ref", "libwarprnnt.so"))):
+    if force or stale or (_ref_sources() and not os.path.exists(os.path.join(_HERE, "_ref", "libwarprnnt.so"))):
         subprocess.run(["make", "-C", _HERE, "all"], check=True, capture_output=True)
     return so
+
+
+def _ref_sources():
+    d = os.environ.get("WARP_TRANSDUCER_DIR")
+    return bool(d) and os.path.isdir(os.path.join(d, "src"))
 
 
 def lib():
@@ -168,7 +172,7 @@ def ref_path():
 
 
 def have_ref():
-    if not os.path.exists(ref_path()) and os.path.isdir("/root/reference/warp-transducer/src"):
+    if not os.path.exists(ref_path()) and _ref_sources():
         build()
     return os.path.exists(ref_path())
 
@@ -177,7 +181,7 @@ def ref():
     global _REF
     if _REF is None:
         if not have_ref():
-            raise FileNotFoundError("oracle/_ref/libwarprnnt.so not built (needs /root/reference)")
+            raise FileNotFoundError("oracle/_ref/libwarprnnt.so not built (set WARP_TRANSDUCER_DIR at build time)")
         L = C.CDLL(ref_path())
         L.rnntGetStatusString.restype = C.c_char_p
         L.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]

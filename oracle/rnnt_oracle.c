@@ -8,8 +8,8 @@
  *
  * Pinning: the float instantiation is checked against (i) the reference's own
  * known-answer tests (warp-transducer/tests/test_cpu.cpp:12-179, tests/test_gpu.cu:96-224,
- * pytorch_binding/test/test.py:51-160) and (ii) the reference library itself built from
- * /root/reference into oracle/_ref/ (see oracle/Makefile) -- tests/test_oracle.py.
+ * pytorch_binding/test/test.py:51-160) and (ii) the reference library itself built into
+ * oracle/_ref/ (see oracle/Makefile), or its stored outputs (tests/golden/ref_cases.npz) -- tests/test_oracle.py.
  * The joint (Dense/tanh/add) has no pinned vectors anywhere in the reference
  * (TensorFlow 2.2 arithmetic, un-vendored): that part is "parity unpinned" and is
  * anchored on model.py:158-166 plus an fp64 torch-autograd cross-check.

@@ -1,6 +1,6 @@
-"""In-tree build of librnnt_b200.so (nvcc cross-compiles sm_100a without a GPU).
+"""In-tree build of librnnt_b200.so for the H100 (nvcc cross-compiles sm_90a without a GPU).
 
-The shared object is git-ignored but travels to the GPU box with the gpurun snapshot.
+The shared object is a build product: git ignores it, `build()` (or `load()` when it is missing) makes it.
 """
 import os
 import shutil
@@ -11,7 +11,7 @@ SRC = os.path.join(HERE, "csrc", "rnnt_b200.cu")
 OUT = os.environ.get("RNNTB200_BUILD_OUT") or os.path.join(HERE, "librnnt_b200.so")
 DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in sorted(os.listdir(os.path.join(HERE, "csrc"))) if f.endswith(".cuh")] + [
     os.path.join(os.path.dirname(HERE), "include", "rnnt_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 
 
@@ -27,7 +27,7 @@ def is_stale():
 
 
 def build(force=False, verbose=False):
-    """Compile csrc/rnnt_b200.cu -> librnnt_b200.so for sm_100a.  Returns the .so path."""
+    """Compile csrc/rnnt_b200.cu -> librnnt_b200.so for sm_90a.  Returns the .so path."""
     if not force and not is_stale():
         return OUT
     if not os.path.exists(nvcc()):

@@ -1,9 +1,8 @@
-// joint_tc.cuh -- tensor-core (tcgen05 / TMEM / TMA) path of the fused joint + loss: shared definitions (tile
+// joint_tc.cuh -- tensor-core (wgmma / TMA / mbarrier) path of the fused joint + loss: shared definitions (tile
 // geometry, kernel parameters, tensor maps, workspace layout, small helper kernels) and the host-side orchestration
-// (tc_forward / tc_backward).  The kernels themselves: joint_tc3.cuh (forward), bwd_tc.cuh (the two backward
-// contractions).  One persistent CTA per SM, each looping over 128-cell lattice tiles (16 time steps x 8 label positions
-// of one utterance); the (B,T,U,H) activation tensor of model.py:158-163 and the (B,T,U,V) logits of model.py:165-166
-// never exist in HBM.
+// (tc_forward / tc_backward).  The kernels themselves: joint_fwd.cuh (forward), joint_bwd.cuh (the two backward
+// contractions).  Persistent CTAs loop over 128-cell lattice tiles (16 time steps x 8 label positions of one utterance);
+// the (B,T,U,H) activation tensor of model.py:158-163 and the (B,T,U,V) logits of model.py:165-166 never exist in HBM.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -23,7 +22,8 @@
 namespace rb {
 
 constexpr int TC_MAX_KB = 16;        // H <= 1024
-constexpr int TC_TMEM_COLS = 512;
+constexpr size_t TC_SMEM_OPTIN = 232448;   // largest dynamic shared memory a block may opt in to (sm_90: 227 KB)
+constexpr int TC_SMS = 132;               // SM count the split-K workspace is sized for (H100 SXM); launches query the device
 
 struct TcGeom {
     int TT, UU, nTb, nUb;  // tile = TT x UU cells (TT*UU == 128); tiles per utterance
@@ -31,10 +31,8 @@ struct TcGeom {
     bool ok;
 };
 
-// Tile shape: 16 time steps x 8 label positions.  (Round 1 picked, per problem, the power-of-two shape with the least
-// padding; every tile re-reads its TT enc rows and UU pred rows (fp32, H wide) from L2, so a balanced shape also
-// minimises that stream: 1 x 128 tiles cost 330 KB per tile, 16 x 8 cost 61 KB.  The backward kernels reduce a tile
-// over u and over t in registers, which fixes the lane <-> (t, u) mapping, so the whole path now uses 16 x 8.)
+// Tile shape: 16 time steps x 8 label positions.  Every tile re-reads its TT enc rows and UU pred rows (fp32, H wide)
+// from L2, so a balanced shape minimises that stream (1 x 128 tiles would cost 330 KB per tile, 16 x 8 cost 61 KB).
 inline TcGeom tc_geometry(int maxT, int maxU, int H, int V) {
     TcGeom g{};
     g.ok = false;
@@ -52,83 +50,22 @@ inline TcGeom tc_geometry(int maxT, int maxU, int H, int V) {
 inline int tc_num_sms() {
     int dev = 0, n = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-        n = 148;
+        n = TC_SMS;
     return n;
-}
-
-// Geometry of the two backward kernels (bwd_tc.cuh), a pure function of (H, V) and the SM count.
-//   dZ: NP passes over H of NCZ columns; accumulators of two consecutive passes share `sh` TMEM columns.
-//   dW: output tiles of (2 block slots of 128 rows out of [H blocks..., ONES]) x 256 columns of V, split S ways over the
-//       lattice rows.
-struct BwdGeom {
-    int NP, NCZ, priv, sh, odd_base, dz_stages;
-    size_t dz_smem, dw_smem;
-    int nVT, nHB, nItems, S_max, dw_grid;     // S_max = the split count S
-    bool ok;
-};
-#ifndef RNNTB200_DZ_EG
-#define RNNTB200_DZ_EG 4
-#endif
-constexpr int RB_DZ_EG = RNNTB200_DZ_EG;      // epilogue warp groups of the dZ kernel (bwd_tc.cuh: DZ_EG)
-// dZ kernel variant: 2 (default) = CTA pairs (cta_group::2, one copy of each W stage per two tiles), 1 = one CTA per tile
-inline int tc_dz_variant() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("RNNTB200_DZ"); v = e ? atoi(e) : 2; if (v != 1 && v != 2) v = 2; }
-    return v;
-}
-// dW kernel variant: 2 (default) = CTA pairs (one z block per CTA against 512 columns), 1 = one CTA per (2 blocks x 256 columns)
-inline int tc_dw_variant() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("RNNTB200_DW"); v = e ? atoi(e) : 2; if (v != 1 && v != 2) v = 2; }
-    return v;
-}
-inline BwdGeom bwd_geometry(int H, int V, int sms = 148, bool dz_pair = true, bool dw_pair = true) {
-    BwdGeom g{};
-    g.ok = false;
-    if (H % 64 || V % 64 || H > 768 || H < 64) return g;
-    g.NP = H <= 384 ? 1 : 2;
-    g.NCZ = H / g.NP;
-    g.sh = 2 * g.NCZ > 512 ? 2 * g.NCZ - 512 : 0;
-    g.priv = g.NCZ - g.sh;
-    g.odd_base = 512 - g.priv;
-    // operand stage: the tile's E' block (16 KB) + the W rows this CTA loads (all NCZ of the pass, or half of them in a pair)
-    const size_t dz_stage = 16384 + (size_t)(dz_pair ? g.NCZ / 2 : g.NCZ) * 128;
-    for (g.dz_stages = dz_pair ? 6 : 3; g.dz_stages >= 2; --g.dz_stages) {
-        g.dz_smem = 1024 + (size_t)g.dz_stages * dz_stage + (size_t)(g.NCZ / 32) * 3072 + (size_t)RB_DZ_EG * 2 * 4 * 8 * 36 * 4 + 512;
-        if (g.dz_smem <= 232448) break;
-    }
-    g.nHB = (H + 127) / 128;
-    g.nItems = (g.nHB + 2) / 2;               // blocks [0 .. nHB-1, ONES] in pairs
-    if (dw_pair) {                            // a cluster of 2 per (512 columns, item, split): bwd_dw2_kernel
-        g.dw_smem = 1024 + (size_t)4 * 49152 + 8 * 256 + 512;
-        g.nVT = (V + 511) / 512;
-        g.S_max = (sms / 2) / (g.nVT * g.nItems);
-        if (g.S_max < 1) g.S_max = 1;
-        g.dw_grid = 2 * g.nVT * g.nItems * g.S_max;
-    } else {
-        g.dw_smem = 1024 + (size_t)3 * 65536 + 8 * 256 + 512;
-        g.nVT = (V + 255) / 256;
-        g.S_max = sms / (g.nVT * g.nItems);
-        if (g.S_max < 1) g.S_max = 1;
-        g.dw_grid = g.nVT * g.nItems * g.S_max;
-    }
-    g.ok = g.dz_smem <= 232448 && g.dw_smem <= 232448;
-    return g;
 }
 
 struct JointTcParams {
     const float* enc; const float* pred; const float* bias;
     const int* labels; const int* xlen; const int* ylen;
     int B, maxT, maxU, H, V, blank;
-    int TT, UU, nTb, nUb, NC, NCH, KB, stages;
+    int TT, UU, nTb, nUb, KB, stages;
     long long SK;
     int b0, nb;                 // utterance range of this launch
     const int* slot;            // tile -> compact row block of the kept arrays (valid tiles only); NULL = tile order
-    int nbuf, ks, dbg;          // TMEM accumulator buffers; K-blocks per W stage; bring-up switches
     float* lse; float* lpb; float* lpl;              // outputs (NULL: a recompute that only wants the kept activations)
-    // MODE 2 (forward that KEEPS its activations): dl receives the softmax numerators 2^(y - gm) as fp16, one row of V
-    // per lattice cell, gm the running maximum each 32-column group was taken against.
-    __nv_bfloat16* dl;          // (16-bit storage; the numerators are fp16)
+    // MODE 2 (forward that KEEPS its activations): dl receives the softmax numerators 2^(y - ref) as bf16, one row of V
+    // per lattice cell, gm the row's reference ref (log2 domain).
+    __nv_bfloat16* dl;
     float* gm;
 };
 struct TileInfo { int b, t0, u0, Tn, Un; bool valid; };
@@ -266,35 +203,6 @@ inline bool make_tmap_bf16(CUtensorMap* tm, const void* base, uint64_t rows, uin
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// W^T (V,H) bf16 viewed as 3-D (k within a 64-wide K block, v, K block): one request brings `kblocks` K-major
-// SWIZZLE_128B slabs [box_rows x 64] that land back to back in shared memory.
-inline bool make_tmap_bf16_kblocks(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                                   uint32_t kblocks) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) return false;
-    cuuint64_t dims[3] = {64, rows, cols / 64};
-    cuuint64_t strides[2] = {cols * 2, 128};
-    cuuint32_t box[3] = {64, box_rows, kblocks};
-    cuuint32_t estr[3] = {1, 1, 1};
-    return fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// 2-D row-major fp32 matrix [rows x cols], box [box_rows x box_cols]; swizzle128 requires box_cols*4 == 128
-inline bool make_tmap_f32(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                          uint32_t box_cols, bool swizzle128) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 4};
-    cuuint32_t box[2] = {box_cols, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // Workspace of the tensor-core path (a pure function of the descriptor).  The kept arrays (numerators + maxima) are
 // laid out per 128-row tile; the batch is processed in utterance chunks that keep them under ~16 GiB.
 struct TcScratch {
@@ -320,66 +228,11 @@ inline size_t tc_chunk_budget() {
     if (!v) { const char* e = getenv("RNNTB200_CHUNK_MB"); v = e && atoll(e) > 0 ? (size_t)atoll(e) << 20 : (size_t)16 << 30; }
     return v;
 }
-inline TcScratch tc_scratch_layout(const rnntb200JointDesc& d, void* base) {
-    TcScratch s{};
-    const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
-    const BwdGeom bg = bwd_geometry(d.H, d.V, 148, tc_dz_variant() == 2, tc_dw_variant() == 2);
-    const size_t rows_utt = (size_t)g.nTb * g.nUb * 128;
-    const size_t per_row = (size_t)d.V * 2 + 8;
-    size_t bc = tc_chunk_budget() / (rows_utt * per_row);
-    if (bc < 1) bc = 1;
-    if (bc > (size_t)d.B) bc = d.B;
-    s.bchunk = (int)bc;
-    s.rows_chunk = bc * rows_utt;
-    // The kept arrays are indexed by COMPACT slots (valid tiles only), but how many tiles are valid is known to the device
-    // alone, so the default sizes them for every tile of the padded (maxT, maxU) lattice and chunks the batch.  A caller
-    // that knows its lengths on the host can promise an upper bound: the whole batch is then ONE chunk of that many row
-    // blocks (C5: 46 k valid of 160 k padded tiles -- keep mode instead of 11 recomputing chunks).
-    if (d.valid_tile_bound > 0 && bc < (size_t)d.B) {
-        const size_t tiles = (size_t)d.valid_tile_bound < (size_t)d.B * g.nTb * g.nUb ? (size_t)d.valid_tile_bound : (size_t)d.B * g.nTb * g.nUb;
-        if (tiles * 128 * per_row <= ((size_t)160 << 30)) { bc = d.B; s.bchunk = d.B; s.rows_chunk = tiles * 128; }
-    }
-    char* p = static_cast<char*>(base);
-    auto take = [&](size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; };
-    s.Wt = reinterpret_cast<__nv_bfloat16*>(take((size_t)d.V * d.H * 2));
-    s.Wb = reinterpret_cast<__nv_bfloat16*>(take((size_t)d.V * d.H * 2));
-    s.dl = reinterpret_cast<__nv_bfloat16*>(take(s.rows_chunk * d.V * 2));
-    s.gm = reinterpret_cast<float*>(take(s.rows_chunk * 4));
-    s.slot = reinterpret_cast<int*>(take((size_t)bc * g.nTb * g.nUb * 4));
-    s.tile_of_slot = reinterpret_cast<int*>(take((size_t)bc * g.nTb * g.nUb * 4));
-    s.slot_meta = reinterpret_cast<int4*>(take((size_t)bc * g.nTb * g.nUb * 16));
-    s.count = reinterpret_cast<int*>(take(256));
-    s.ppl = reinterpret_cast<float*>(take((size_t)g.nTb * bc * d.maxU * d.H * 4));
-    s.dWp = reinterpret_cast<float*>(take((size_t)bg.S_max * d.H * d.V * 4));
-    s.dbp = reinterpret_cast<float*>(take((size_t)bg.S_max * d.V * 4));
-    s.rowscale = reinterpret_cast<float*>(take(s.rows_chunk * 4));
-    s.bytes = (size_t)(p - static_cast<char*>(base));
-    return s;
-}
-
 inline rnntStatus_t tc_unsupported(const rnntb200JointDesc& d) {
     fprintf(stderr,
             "rnnt_b200: RNNTB200_BF16_TC needs H %% 64 == 0, V %% 64 == 0 and 64 <= H <= 768 (got H=%d V=%d); "
             "use RNNTB200_FP32_EXACT\n", d.H, d.V);
     return RNNT_STATUS_INVALID_VALUE;
-}
-
-inline bool tc_fill_params(const rnntb200JointDesc& d, const TcGeom& g, JointTcParams& p, const float* enc,
-                           const float* pred, const float* bias, const int* labels, const int* ylen,
-                           const int* xlen) {
-    p = JointTcParams{};
-    p.enc = enc; p.pred = pred; p.bias = bias; p.labels = labels; p.xlen = xlen; p.ylen = ylen;
-    p.B = d.B; p.maxT = d.maxT; p.maxU = d.maxU; p.H = d.H; p.V = d.V; p.blank = d.blank_label;
-    p.TT = g.TT; p.UU = g.UU; p.nTb = g.nTb; p.nUb = g.nUb; p.KB = g.KB;
-    p.SK = (long long)(d.maxT + d.maxU - 1) * d.maxU;
-    return true;
-}
-
-// RNNTB200_DBG=<bits>: switch kernel roles off for timing experiments (results are wrong by design)
-inline int tc_dbg() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("RNNTB200_DBG"); v = e ? atoi(e) : 0; }
-    return v;
 }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE property of a kernel: set it once per (device, kernel),
@@ -393,35 +246,57 @@ inline bool tc_smem_optin(const void* func) {
     std::lock_guard<std::mutex> lk(mu);
     auto it = done.find(key);
     if (it != done.end()) return true;
-    if (cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448) != cudaSuccess) return false;
+    if (cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_OPTIN) != cudaSuccess) return false;
     done[key] = true;
     return true;
 }
 
 }  // namespace rb
 
-#include "joint_tc3.cuh"
-#include "joint_tc4.cuh"
-#include "bwd_tc.cuh"
+#include "joint_fwd.cuh"
+#include "joint_bwd.cuh"
 
 namespace rb {
 
-// RNNTB200_PROF=1 (bring-up): the backward kernels record per-role wait cycles into a managed buffer that
-// rnntb200_debug_prof() exposes (tools/role_profile.py); off by default, never touched otherwise.
-inline long long* tc_prof_buffer(int which) {
-    static long long* buf[2] = {nullptr, nullptr};
-    static int on = -1;
-    if (on < 0) { const char* e = getenv("RNNTB200_PROF"); on = e ? atoi(e) : 0; }
-    if (!on) return nullptr;
-    if (!buf[which]) {
-        if (cudaMallocManaged(reinterpret_cast<void**>(&buf[which]), sizeof(long long) * 256 * 4 * 8) != cudaSuccess) return nullptr;
-        cudaMemset(buf[which], 0, sizeof(long long) * 256 * 4 * 8);
+inline TcScratch tc_scratch_layout(const rnntb200JointDesc& d, void* base) {
+    TcScratch s{};
+    const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
+    const DwGeom wg = dw_geometry(d.H, d.V);
+    const size_t rows_utt = (size_t)g.nTb * g.nUb * 128;
+    const size_t per_row = (size_t)d.V * 2 + 8;
+    size_t bc = tc_chunk_budget() / (rows_utt * per_row);
+    if (bc < 1) bc = 1;
+    if (bc > (size_t)d.B) bc = d.B;
+    s.bchunk = (int)bc;
+    s.rows_chunk = bc * rows_utt;
+    // The kept arrays are indexed by COMPACT slots (valid tiles only), but how many tiles are valid is known to the device
+    // alone, so the default sizes them for every tile of the padded (maxT, maxU) lattice and chunks the batch.  A caller
+    // that knows its lengths on the host can promise an upper bound: the whole batch is then ONE chunk of that many row
+    // blocks, as long as they fit in 56 GiB (an 80 GB device also holds the inputs, the loss planes and the gradients).
+    if (d.valid_tile_bound > 0 && bc < (size_t)d.B) {
+        const size_t tiles = (size_t)d.valid_tile_bound < (size_t)d.B * g.nTb * g.nUb ? (size_t)d.valid_tile_bound : (size_t)d.B * g.nTb * g.nUb;
+        if (tiles * 128 * per_row <= ((size_t)56 << 30)) { bc = d.B; s.bchunk = d.B; s.rows_chunk = tiles * 128; }
     }
-    return buf[which];
+    char* p = static_cast<char*>(base);
+    auto take = [&](size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; };
+    s.Wt = reinterpret_cast<__nv_bfloat16*>(take((size_t)d.V * d.H * 2));
+    s.Wb = reinterpret_cast<__nv_bfloat16*>(take((size_t)d.V * d.H * 2));
+    s.dl = reinterpret_cast<__nv_bfloat16*>(take(s.rows_chunk * d.V * 2));
+    s.gm = reinterpret_cast<float*>(take(s.rows_chunk * 4));
+    s.slot = reinterpret_cast<int*>(take((size_t)bc * g.nTb * g.nUb * 4));
+    s.tile_of_slot = reinterpret_cast<int*>(take((size_t)bc * g.nTb * g.nUb * 4));
+    s.slot_meta = reinterpret_cast<int4*>(take((size_t)bc * g.nTb * g.nUb * 16));
+    s.count = reinterpret_cast<int*>(take(256));
+    s.ppl = reinterpret_cast<float*>(take((size_t)g.nTb * bc * d.maxU * d.H * 4));
+    s.dWp = reinterpret_cast<float*>(take((size_t)wg.S * d.H * d.V * 4));
+    s.dbp = reinterpret_cast<float*>(take((size_t)wg.S * d.V * 4));
+    s.rowscale = reinterpret_cast<float*>(take(s.rows_chunk * 4));
+    s.bytes = (size_t)(p - static_cast<char*>(base));
+    return s;
 }
 
 inline bool tc_supported(const rnntb200JointDesc& d) {
-    return tc_geometry(d.maxT, d.maxU, d.H, d.V).ok && tc3_geometry(d.H, d.V).ok && bwd_geometry(d.H, d.V, 148, tc_dz_variant() == 2, tc_dw_variant() == 2).ok;
+    return tc_geometry(d.maxT, d.maxU, d.H, d.V).ok && d.H <= 768 && fwd_geometry(d.H, d.V).ok && dz_geometry(d.H).ok;
 }
 inline size_t tc_scratch_bytes(const rnntb200JointDesc& d) {
     if (!tc_supported(d)) return 0;
@@ -436,28 +311,22 @@ inline bool tc_keep(const rnntb200JointDesc& d, const TcScratch& sc) {
     return d.keep_activations && env && sc.bchunk >= d.B;
 }
 
-// RNNTB200_FWD=3|4: forward kernel generation (4 = CTA pairs, the default; 3 = one CTA per tile, kept for A/B measurements)
-inline int tc_fwd_variant() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("RNNTB200_FWD"); v = e ? atoi(e) : 4; if (v != 3 && v != 4) v = 4; }
-    return v;
-}
-
 // the forward kernel over utterances [b0, b0+nb); KEEP: rank the chunk's valid tiles on the device (nothing is read
-// back) and leave numerators + maxima in the workspace
+// back) and leave numerators + references in the workspace
 template <bool KEEP>
 inline rnntStatus_t tc_run_forward(const rnntb200JointDesc& d, const TcGeom& g, const TcScratch& sc, const float* enc,
                                    const float* pred, const float* bias, const int* labels, const int* ylen,
                                    const int* xlen, float* lse, float* lpb, float* lpl, int b0, int nb, cudaStream_t s,
                                    unsigned* launches) {
-    const bool pair = tc_fwd_variant() == 4;             // CTA-pair kernel (joint_tc4.cuh) or one CTA per tile (joint_tc3.cuh)
-    const Tc2Geom g3 = pair ? tc4_geometry(d.H, d.V) : tc3_geometry(d.H, d.V);
-    JointTcParams p;
-    tc_fill_params(d, g, p, enc, pred, bias, labels, ylen, xlen);
+    const FwdGeom fg = fwd_geometry(d.H, d.V);
+    JointTcParams p{};
+    p.enc = enc; p.pred = pred; p.bias = bias; p.labels = labels; p.xlen = xlen; p.ylen = ylen;
+    p.B = d.B; p.maxT = d.maxT; p.maxU = d.maxU; p.H = d.H; p.V = d.V; p.blank = d.blank_label;
+    p.TT = g.TT; p.UU = g.UU; p.nTb = g.nTb; p.nUb = g.nUb; p.KB = g.KB;
+    p.SK = (long long)(d.maxT + d.maxU - 1) * d.maxU;
     p.b0 = b0; p.nb = nb;
     p.lse = lse; p.lpb = lpb; p.lpl = lpl;
-    p.NC = TC2_NC; p.NCH = d.V / TC2_NC; p.stages = g3.stages; p.nbuf = g3.nbuf; p.ks = g3.ks;
-    p.dbg = tc_dbg();
+    p.stages = fg.stages;
     if (KEEP) {
         const int ntiles = nb * g.nTb * g.nUb;
         tile_compact_kernel<<<1, 1024, 0, s>>>(xlen, ylen, b0, ntiles, g.nTb, g.nUb, g.TT, g.UU, sc.slot, sc.count, sc.tile_of_slot, sc.slot_meta,
@@ -465,16 +334,13 @@ inline rnntStatus_t tc_run_forward(const rnntb200JointDesc& d, const TcGeom& g, 
         *launches += 1;
         p.slot = sc.slot; p.dl = sc.dl; p.gm = sc.gm;
     }
-    CUtensorMap tm, tmp, tme;
-    if (!make_tmap_bf16_kblocks(&tm, sc.Wt, d.V, d.H, pair ? TC2_NC / 2 : TC2_NC, g3.ks) ||
-        !make_tmap_f32(&tmp, pred, (uint64_t)d.B * d.maxU, d.H, g.UU, 32, true) ||
-        !make_tmap_f32(&tme, enc, (uint64_t)d.B * d.maxT, d.H, g.TT, 64, false)) {
+    CUtensorMap tm;
+    if (!make_tmap_bf16(&tm, sc.Wt, d.V, d.H, FWD_NC)) {
         fprintf(stderr, "rnnt_b200: cuTensorMapEncodeTiled failed\n");
         return RNNT_STATUS_EXECUTION_FAILED;
     }
     *launches += 1;
-    if (pair) return tc4_launch<KEEP ? 2 : 0>(g3, tm, tmp, tme, p, s);
-    return tc3_launch<KEEP ? 2 : 0>(g3, tm, tmp, tme, p, s);
+    return fwd_launch<KEEP ? 2 : 0>(fg, tm, p, s);
 }
 
 inline rnntStatus_t tc_forward(const rnntb200JointDesc& d, void* scratch, const float* enc, const float* pred,
@@ -493,9 +359,9 @@ inline rnntStatus_t tc_forward(const rnntb200JointDesc& d, void* scratch, const 
 
 struct LossPlanes { const float *lse, *lpb, *lpl, *alphas, *betas, *llf; };   // outputs of the forward + alpha/beta (loss workspace)
 
-// Backward (SURVEY 8 a19) with the library's own tcgen05 kernels (bwd_tc.cuh).  Per utterance chunk: (a keeping
-// forward of the chunk unless the forward call already kept the whole batch) -> bwd_dz_kernel -> d_pred plane sum ->
-// bwd_dw_kernel; after the last chunk the split-K planes of dW / db are summed.  Stream-ordered, no host
+// Backward (SURVEY 8 a19) with the library's own wgmma kernels (joint_bwd.cuh).  Per utterance chunk: (a keeping forward
+// of the chunk unless the forward call already kept the whole batch) -> row_scale_kernel -> bwd_dz_kernel -> d_pred plane
+// sum -> bwd_dw_kernel; after the last chunk the split-K planes of dW / db are summed.  Stream-ordered, no host
 // synchronisation, no library calls.
 inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const float* enc, const float* pred,
                                 const float* bias, const int* labels, const int* ylen, const int* xlen,
@@ -503,24 +369,18 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
                                 float* db, cudaStream_t s, unsigned* launches) {
     if (!tc_supported(d)) return tc_unsupported(d);
     const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
-    const bool dz_pair = tc_dz_variant() == 2, dw_pair = tc_dw_variant() == 2;
-    const BwdGeom bg = bwd_geometry(d.H, d.V, 148, dz_pair, dw_pair);
+    const DzGeom zg = dz_geometry(d.H);
+    const DwGeom wg = dw_geometry(d.H, d.V);
     TcScratch sc = tc_scratch_layout(d, scratch);   // Wt / Wb were produced by the forward call
     const bool kept = tc_keep(d, sc);
-    if (!tc_smem_optin(reinterpret_cast<const void*>(bwd_dz_kernel<false, false>)) || !tc_smem_optin(reinterpret_cast<const void*>(bwd_dz_kernel<true, false>)) ||
-        !tc_smem_optin(reinterpret_cast<const void*>(bwd_dz_kernel<false, true>)) || !tc_smem_optin(reinterpret_cast<const void*>(bwd_dz_kernel<true, true>)) ||
-        !tc_smem_optin(reinterpret_cast<const void*>(bwd_dw_kernel<false>)) || !tc_smem_optin(reinterpret_cast<const void*>(bwd_dw_kernel<true>)) ||
-        !tc_smem_optin(reinterpret_cast<const void*>(bwd_dw2_kernel<false>)) || !tc_smem_optin(reinterpret_cast<const void*>(bwd_dw2_kernel<true>)))
+    if (!tc_smem_optin(reinterpret_cast<const void*>(bwd_dz_kernel)) || !tc_smem_optin(reinterpret_cast<const void*>(bwd_dw_kernel)))
         return RNNT_STATUS_EXECUTION_FAILED;
-    if (cudaMemsetAsync(sc.dWp, 0, sizeof(float) * (size_t)bg.S_max * d.H * d.V, s) != cudaSuccess ||
-        cudaMemsetAsync(sc.dbp, 0, sizeof(float) * (size_t)bg.S_max * d.V, s) != cudaSuccess)
+    if (cudaMemsetAsync(sc.dWp, 0, sizeof(float) * (size_t)wg.S * d.H * d.V, s) != cudaSuccess ||
+        cudaMemsetAsync(sc.dbp, 0, sizeof(float) * (size_t)wg.S * d.V, s) != cudaSuccess)
         return RNNT_STATUS_MEMOPS_FAILED;
-    CUtensorMap tm_e128, tm_e64, tm_wp, tm_ws, tm_p32, tm_e32;
-    if (!make_tmap_f32(&tm_p32, pred, (uint64_t)d.B * d.maxU, d.H, BW_UU, 32, true) ||
-        !make_tmap_f32(&tm_e32, enc, (uint64_t)d.B * d.maxT, d.H, BW_TT, 32, false) ||
-        !make_tmap_bf16(&tm_e128, sc.dl, sc.rows_chunk, d.V, 128) || !make_tmap_bf16(&tm_e64, sc.dl, sc.rows_chunk, d.V, 64) ||
-        !make_tmap_bf16(&tm_wp, sc.Wb, d.H, d.V, dz_pair ? bg.priv / 2 : bg.priv) ||
-        !make_tmap_bf16(&tm_ws, sc.Wb, d.H, d.V, bg.sh ? (dz_pair ? bg.sh / 2 : bg.sh) : 8)) {
+    CUtensorMap tm_e128, tm_e64, tm_w;
+    if (!make_tmap_bf16(&tm_e128, sc.dl, sc.rows_chunk, d.V, 128) || !make_tmap_bf16(&tm_e64, sc.dl, sc.rows_chunk, d.V, 64) ||
+        !make_tmap_bf16(&tm_w, sc.Wb, d.H, d.V, DZ_NC)) {
         fprintf(stderr, "rnnt_b200: cuTensorMapEncodeTiled failed\n");
         return RNNT_STATUS_EXECUTION_FAILED;
     }
@@ -531,10 +391,6 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
             rnntStatus_t st = tc_run_forward<true>(d, g, sc, enc, pred, bias, labels, ylen, xlen, nullptr, nullptr, nullptr, b0, nb, s, launches);
             if (st) return st;
         }
-        BwdParams p{};
-        p.enc = enc; p.pred = pred; p.xlen = xlen; p.ylen = ylen;
-        p.maxT = d.maxT; p.maxU = d.maxU; p.H = d.H; p.V = d.V;
-        p.nTb = g.nTb; p.nUb = g.nUb; p.b0 = b0; p.nb = nb;
         {   // per-row scales of this chunk (row order of the kept arrays) + the two special columns of every row
             ScopedTimer tmr("row_scale_kernel", s);
             row_scale_kernel<<<(unsigned)(((size_t)nb * g.nTb * g.nUb * 128 + 255) / 256), 256, 0, s>>>(
@@ -543,32 +399,20 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
                 d.V, reinterpret_cast<unsigned short*>(sc.dl), sc.rowscale);
             *launches += 1;
         }
-        p.slot = sc.slot; p.tile_of_slot = sc.tile_of_slot; p.slot_meta = sc.slot_meta; p.count = sc.count; p.rowscale = sc.rowscale;
-        p.NP = bg.NP; p.NCZ = bg.NCZ; p.priv = bg.priv; p.sh = bg.sh; p.odd_base = bg.odd_base; p.dz_stages = bg.dz_stages;
-        p.d_enc = d_enc; p.ppred = sc.ppl;
-        p.nVT = bg.nVT; p.nItems = bg.nItems; p.nHB = bg.nHB; p.S = bg.S_max; p.Hrows = d.H;
-        p.dWp = sc.dWp; p.dbp = sc.dbp;
-        long long* prof_dz = tc_prof_buffer(0), *prof_dw = tc_prof_buffer(1);
+        BwdParams p{};
+        p.enc = enc; p.pred = pred; p.xlen = xlen; p.ylen = ylen;
+        p.maxT = d.maxT; p.maxU = d.maxU; p.H = d.H; p.V = d.V;
+        p.nTb = g.nTb; p.nUb = g.nUb; p.b0 = b0; p.nb = nb;
+        p.slot = sc.slot; p.slot_meta = sc.slot_meta; p.count = sc.count; p.rowscale = sc.rowscale;
+        p.dz_stages = zg.stages; p.d_enc = d_enc; p.ppred = sc.ppl;
+        p.nVT = wg.nVT; p.nHB = wg.nHB; p.S = wg.S; p.dWp = sc.dWp; p.dbp = sc.dbp;
         // rows of d_enc whose t-block lies outside the utterance are never visited by the dZ kernel
         if (cudaMemsetAsync(d_enc + (size_t)b0 * d.maxT * d.H, 0, sizeof(float) * (size_t)nb * d.maxT * d.H, s) != cudaSuccess)
             return RNNT_STATUS_MEMOPS_FAILED;
         {
             const int nruns = nb * g.nTb;
             ScopedTimer tmr("bwd_dz_kernel", s);
-            p.prof = prof_dz;
-            if (dz_pair) {
-                const int npairs = nruns < sms / 2 ? nruns : sms / 2;
-                cudaLaunchConfig_t cfg{};
-                cfg.gridDim = dim3(2 * npairs); cfg.blockDim = dim3(DZ_THREADS); cfg.dynamicSmemBytes = bg.dz_smem; cfg.stream = s;
-                cudaLaunchAttribute at[1];
-                at[0].id = cudaLaunchAttributeClusterDimension;
-                at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-                cfg.attrs = at; cfg.numAttrs = 1;
-                if (cudaLaunchKernelEx(&cfg, p.prof ? bwd_dz_kernel<true, true> : bwd_dz_kernel<false, true>, tm_e128, tm_wp, tm_ws, tm_p32,
-                                       tm_e32, p) != cudaSuccess)
-                    return RNNT_STATUS_EXECUTION_FAILED;
-            } else if (p.prof) bwd_dz_kernel<true, false><<<nruns < sms ? nruns : sms, DZ_THREADS, bg.dz_smem, s>>>(tm_e128, tm_wp, tm_ws, tm_p32, tm_e32, p);
-            else bwd_dz_kernel<false, false><<<nruns < sms ? nruns : sms, DZ_THREADS, bg.dz_smem, s>>>(tm_e128, tm_wp, tm_ws, tm_p32, tm_e32, p);
+            bwd_dz_kernel<<<nruns < sms ? nruns : sms, BWD_THREADS, zg.smem_bytes, s>>>(tm_e128, tm_w, p);
         }
         {
             const size_t n4 = (size_t)nb * d.maxU * d.H / 4;
@@ -577,13 +421,8 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
                 reinterpret_cast<const float4*>(sc.ppl), xlen, ylen, b0, nb, d.maxU, d.H / 4, reinterpret_cast<float4*>(d_pred));
         }
         {
-            ScopedTimer tmr(dw_pair ? "bwd_dw2_kernel" : "bwd_dw_kernel", s);
-            p.prof = prof_dw;
-            if (dw_pair) {
-                if (p.prof) bwd_dw2_kernel<true><<<bg.dw_grid, DW_THREADS, bg.dw_smem, s>>>(tm_e64, p);
-                else bwd_dw2_kernel<false><<<bg.dw_grid, DW_THREADS, bg.dw_smem, s>>>(tm_e64, p);
-            } else if (p.prof) bwd_dw_kernel<true><<<bg.dw_grid, DW_THREADS, bg.dw_smem, s>>>(tm_e64, p);
-            else bwd_dw_kernel<false><<<bg.dw_grid, DW_THREADS, bg.dw_smem, s>>>(tm_e64, p);
+            ScopedTimer tmr("bwd_dw_kernel", s);
+            bwd_dw_kernel<<<wg.nVT * wg.nHB * wg.S, BWD_THREADS, wg.smem_bytes, s>>>(tm_e64, p);
         }
         *launches += 3;
         if (cudaGetLastError() != cudaSuccess) return RNNT_STATUS_EXECUTION_FAILED;
@@ -592,12 +431,11 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         ScopedTimer tmr("sum_planes_kernel", s);
         const size_t nw4 = (size_t)d.H * d.V / 4, nb4 = (size_t)d.V / 4;
         sum_planes_kernel<<<(unsigned)((nw4 + 255) / 256 < 4096 ? (nw4 + 255) / 256 : 4096), 256, 0, s>>>(
-            reinterpret_cast<const float4*>(sc.dWp), bg.S_max, nw4, reinterpret_cast<float4*>(dW));
-        sum_planes_kernel<<<(unsigned)((nb4 + 255) / 256), 256, 0, s>>>(reinterpret_cast<const float4*>(sc.dbp), bg.S_max, nb4,
+            reinterpret_cast<const float4*>(sc.dWp), wg.S, nw4, reinterpret_cast<float4*>(dW));
+        sum_planes_kernel<<<(unsigned)((nb4 + 255) / 256), 256, 0, s>>>(reinterpret_cast<const float4*>(sc.dbp), wg.S, nb4,
                                                                        reinterpret_cast<float4*>(db));
     }
     *launches += 2;
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
 }
-
 }  // namespace rb

@@ -1,4 +1,4 @@
-// kernels_simt.cuh -- CUDA-core kernels of the RNN-T loss hot path (sm_100a).
+// kernels_simt.cuh -- CUDA-core kernels of the RNN-T loss hot path (sm_90a).
 //
 //   lse_gather_kernel   log-softmax denominators + (blank, label) log-prob gather, one pass
 //                       (replaces reduce_max + reduce_exp + logp(): gpu_rnnt.h:73-80,

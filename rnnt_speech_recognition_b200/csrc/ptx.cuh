@@ -1,7 +1,7 @@
-// ptx.cuh -- thin inline-PTX wrappers for the Blackwell (sm_100a) features the joint kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences) and the
-// UMMA shared-memory / instruction descriptors.  Bit layouts follow the PTX ISA tcgen05 chapter
-// (cross-checked against cute/arch/mma_sm100_desc.hpp: SmemDescriptor, InstrDescriptor).
+// ptx.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) features the joint kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors) and its
+// shared-memory matrix descriptor.  Bit layouts follow the PTX ISA "Asynchronous Warpgroup Level Matrix"
+// chapter (matrix descriptor format, canonical swizzled layouts).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,7 @@ __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
     __syncwarp();
 }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ------------------------------------------------------------------ TMA
@@ -75,180 +75,67 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05: TMEM allocation
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp, .sync.aligned
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ------------------------------------------------------------------ tcgen05: descriptors
-// Shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, 16-bit elements:
-//   rows of 64 elements (128 B), 8-row core groups 1024 B apart (SBO), base 1024-B aligned.
-//   bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2 (SW128)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor (sm_90 GmmaDescriptor), SWIZZLE_128B, 16-bit elements, base 1024-B aligned:
+//   bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (SW128)
+// K-major operand: rows of 64 elements (128 B), 8-row core groups SBO = 1024 B apart, LBO unused; a K step of 16 elements
+// advances the start address by 32 B inside the swizzled row.
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;              // LBO (unused for swizzled K-major), canonical value 1
-    d |= (uint64_t)(1024 >> 4) << 32;    // SBO = 1024 B
-    d |= (uint64_t)1 << 46;              // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;              // SWIZZLE_128B
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// MN-major operand, SWIZZLE_128B, 16-bit elements: 64 MN-elements (128 B) contiguous per K row,
-// 8 K-rows per 1024-B core group (SBO = 1024), next 64 MN-elements `lbo_bytes` away.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+// MN-major operand: 64 MN-elements (128 B) contiguous per K row, 8 K rows per 1024-B core group (SBO = 1024), the next 64
+// MN-elements `lbo_bytes` away; a K step of 16 rows advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// Instruction descriptor, kind::f16: D=f32, A=B=bf16, dense, no negate.
-//   [4,6) c_format=1 (F32) | [7,10) a_format=1 (BF16) | [10,13) b_format=1 | [15] a_major | [16] b_major
-//   | [17,23) N>>3 | [24,29) M>>4          (major: 0 = K-major, 1 = MN-major)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads of an accumulator above the wgmma_wait that makes it valid
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Accumulator fragment of m64nNk16 (f32): thread t of the warpgroup holds d[i] at
+//   row = 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),  column = 8 * (i / 4) + 2 * (t % 4) + (i % 2).
+// D[64 x 64] (+)= A[64 x 16] . B[16 x 64], fp16 operands from shared memory (B MN-major when TRANS_B)
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n64_f16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, %35;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TRANS_B));
+}
+// D[64 x 128] (+)= A[64 x 16] . B[16 x 128], bf16 operands from shared memory (B MN-major when TRANS_B)
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n128_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, %67;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TRANS_B));
 }
 
-// same, A = B = fp16 (a_format = b_format = 0)
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] . B[smem]^T ; single-thread issue
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem]^T : A is read from tensor memory (lane = row, 16-bit K elements packed two
-// per 32-bit column), B through a shared-memory descriptor
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued tcgen05.mma of this thread complete -> one arrive on the mbarrier
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// ------------------------------------------------------------------ CTA pairs (cluster of 2, tcgen05 cta_group::2)
-// Validated on B200 by tools/probes/mma2_probe (profiles/r02/mma2_probe.log): exact accumulators in both CTAs, 32.1 cycles
-// per M=256 N=64 K=16 instruction.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `p` (a shared-memory object of THIS CTA's layout) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
-    return r;
-}
-// (default .release.cta semantics: what crosses the pair here are tcgen05 reads / writes, ordered by tcgen05.fence; a
-//  .release.cluster arrive costs a cluster-scope fence -- L1 invalidation -- on every handshake: measured +1.2 ms per launch)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMEM management for a CTA pair: the SAME warp of BOTH CTAs executes these
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[tmem of each CTA] . B[smem halves of both CTAs]^T, M = 256; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_ts2(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem, 128 rows in each CTA] . B[smem, N/2 rows in each CTA]^T, M = 256 (descriptors are CTA-local
-// offsets, applied in both CTAs)
-__device__ __forceinline__ void umma_ss2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued cta_group::2 MMAs of this thread complete -> one arrive on the barrier at this offset in every CTA of the mask
-__device__ __forceinline__ void umma_commit2_mc(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(cta_mask) : "memory");
-}
-// 3-D tiled load into THIS CTA's shared memory whose bytes are counted on an mbarrier given by its shared::cluster address
-// (the leader's barrier collects both halves of a pair's operand stage)
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05: TMEM -> registers
-// 32 lanes x 32 consecutive 32-bit columns; thread i of the warp receives lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// registers -> TMEM: 32 lanes x 16 consecutive 32-bit columns; thread i writes lane (base_lane + i)
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ explicit shared-memory accesses
 // The kernels carve their dynamic shared memory from a 1024-byte aligned base computed through uintptr_t, which makes the
@@ -316,12 +203,6 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {   // lo -> 
 }
 __device__ __forceinline__ void unpack_f16x2(uint32_t w, float& lo, float& hi) {
     asm("{\n.reg .f16 l, h;\nmov.b32 {l, h}, %2;\ncvt.f32.f16 %0, l;\ncvt.f32.f16 %1, h;\n}" : "=f"(lo), "=f"(hi) : "r"(w));
-}
-// 32 bytes per lane in one request (sm_100: STG.256).  Stores whose lanes hit 32 different rows cost one LSU wavefront
-// per lane whatever their width, so doubling the width halves the wavefronts of such a scattered tile write.
-__device__ __forceinline__ void st_global_256(void* p, const uint32_t* v) {   // p 32-byte aligned, v[0..7]
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 :: "l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
 }
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;

@@ -1,5 +1,5 @@
 // rnnt_b200.cu -- C ABI (include/rnnt_b200.h) and host-side orchestration of the RNN-T loss hot
-// path on B200.  No allocation, no host synchronisation (except the reference-mandated one in
+// path on H100 (sm_90a).  No allocation, no host synchronisation (except the reference-mandated one in
 // compute_rnnt_loss), everything stream-ordered on the caller's stream.
 #include "../../include/rnnt_b200.h"
 
@@ -190,7 +190,7 @@ bool desc_ok(const rnntb200JointDesc* d) {
 
 inline unsigned ew_blocks(long long total) {
     long long b = (total + 255) / 256;
-    return (unsigned)(b > 148 * 32 ? 148 * 32 : (b < 1 ? 1 : b));
+    return (unsigned)(b > 132 * 32 ? 132 * 32 : (b < 1 ? 1 : b));
 }
 
 // C[M,N] (+)= A.B with generic strides; picks the 128x128 float4 kernel when alignment allows
@@ -202,12 +202,12 @@ void launch_sgemm(const float* A, const float* Bm, float* C, const float* bias, 
     const bool b_ok = BN_ ? (N % 4 == 0 && sBk % 4 == 0) : (K % 4 == 0 && sBn % 4 == 0);
     const bool fast = a_ok && b_ok && N % 4 == 0 && ldc % 4 == 0 && al16(A) && al16(Bm) && al16(C) && (!bias || al16(bias));
     if (fast) {
-        // few output tiles but a long K (dW = Z^T.dL): split K over blockIdx.z so the grid fills the 148 SMs;
+        // few output tiles but a long K (dW = Z^T.dL): split K over blockIdx.z so the grid fills the 132 SMs;
         // only for accumulating calls, whose output already holds valid data to atomically add into
         int splits = 1;
         const int tiles = ((N + 127) / 128) * ((M + 127) / 128);
-        if (accumulate && tiles < 148 && K >= 4096) {
-            splits = (148 * 4 + tiles - 1) / tiles;
+        if (accumulate && tiles < 132 && K >= 4096) {
+            splits = (132 * 4 + tiles - 1) / tiles;
             if (splits > K / 512) splits = K / 512;
             if (splits < 1) splits = 1;
         }
@@ -377,7 +377,7 @@ rnntStatus_t rnntb200_joint_loss_forward(const rnntb200JointDesc* desc, const fl
                             ws.loss.lpb, ws.loss.lpl, s, &nl);
         RB_LAUNCHED(nl);
 #else
-        fprintf(stderr, "rnnt_b200: built without the tcgen05 path\n");
+        fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
         st = RNNT_STATUS_EXECUTION_FAILED;
 #endif
     }
@@ -418,7 +418,7 @@ rnntStatus_t rnntb200_joint_loss_backward(const rnntb200JointDesc* desc, const f
     RB_LAUNCHED(nl);
     return st;
 #else
-    fprintf(stderr, "rnnt_b200: built without the tcgen05 path\n");
+    fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
     return RNNT_STATUS_EXECUTION_FAILED;
 #endif
 }
@@ -490,11 +490,6 @@ rnntStatus_t rnntb200_dense1_backward(const float* X, const float* dA, const flo
     return check_launch();
 }
 
-#ifndef RNNTB200_NO_TC
-// bring-up only (not in the public header): role wait-cycle counters of the last backward launch, see tc_prof_buffer()
-const long long* rnntb200_debug_prof(int which) { return rb::tc_prof_buffer(which); }
-#endif
-
 unsigned long long rnntb200_launch_count() { return g_launches.load(); }
 
 void rnntb200_set_timing(int on) { rb::timing_reset(on); }
@@ -509,9 +504,9 @@ int rnntb200_get_timing(int index, const char** name, float* ms) {
 
 const char* rnntb200_build_info() {
 #ifndef RNNTB200_NO_TC
-    return "rnnt_b200 0.1 sm_100a tcgen05=1";
+    return "rnnt_b200 0.1 sm_90a wgmma=1";
 #else
-    return "rnnt_b200 0.1 sm_100a tcgen05=0";
+    return "rnnt_b200 0.1 sm_90a wgmma=0";
 #endif
 }
 

@@ -1,13 +1,18 @@
-// Link-level check of the drop-in boundary: this translation unit includes the REFERENCE's own header
-// (warp-transducer/include/rnnt.h, found through -I at build time -- it is not copied into this repo) and is linked
-// against librnnt_b200.so.  It is what a binding such as tensorflow_binding/src/warprnnt_op.cc:105-141 or
+// Link-level check of the drop-in boundary: this translation unit is written against the warp-transducer C API and
+// linked against librnnt_b200.so.  It includes the library's public header include/rnnt_b200.h, or -- when the build
+// is pointed at a warp-transducer checkout (WARP_TRANSDUCER_DIR, -DRNNT_REFERENCE_HEADER) -- that project's own
+// include/rnnt.h, which is never copied into this repo.  It is what a binding such as tensorflow_binding/src/warprnnt_op.cc:105-141 or
 // pytorch_binding/src/binding.cpp:84-154 does with the library: get_workspace_size -> device workspace ->
 // compute_rnnt_loss(RNNT_GPU, device labels/lengths, HOST costs) -> status string.
 // Data: the reference's own known-answer test (tests/test_cpu.cpp:12-71 / test_gpu.cu small_test): B=1 T=2 U=3 V=5,
 // expected cost 4.495666 and the logits gradient of pytorch_binding/test/test.py:62-74.
 // Modes:  abi_harness link   -> resolves every symbol and checks the host-only entry points (no GPU needed)
 //         abi_harness run    -> runs the KAT on cuda:0
+#ifdef RNNT_REFERENCE_HEADER
 #include <rnnt.h>
+#else
+#include "../../include/rnnt_b200.h"
+#endif
 
 #include <cuda_runtime.h>
 

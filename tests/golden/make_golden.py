@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate the committed golden fixtures under tests/golden/ FROM THE REFERENCE.
 
-Run in the build container only (needs /root/reference); the outputs (*.npz) are committed so
-that nothing on the GPU box reads /root/reference.
+Needs a warp-transducer checkout (WARP_TRANSDUCER_DIR); the outputs (*.npz) are committed so that
+the tests never read the reference sources.
 
 Sources of truth, in order:
   1. The reference's own known-answer tests, parsed (not hand-copied) from
@@ -31,7 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 from oracle import oracle  # noqa: E402
 
-REF = "/root/reference/warp-transducer"
+REF = os.environ.get("WARP_TRANSDUCER_DIR", "warp-transducer")
 
 
 # ------------------------------------------------------------------ 1. parse the reference KATs

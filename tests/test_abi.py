@@ -85,8 +85,8 @@ def test_struct_layout_matches_reference_header():
 
 
 def test_reference_header_links_against_this_library():
-    """Header-level ABI check: tests/abi_harness/abi_harness.cpp includes the REFERENCE's rnnt.h (never copied here) and
-    is linked against librnnt_b200.so -- what tensorflow_binding/src/warprnnt_op.cc:105-141 and
+    """Header-level ABI check: tests/abi_harness/abi_harness.cpp, written against the warp-transducer C API (rnnt.h when
+    the build is given a warp-transducer checkout, the library's own header otherwise), is linked against librnnt_b200.so -- what tensorflow_binding/src/warprnnt_op.cc:105-141 and
     pytorch_binding/src/binding.cpp:84-154 do.  `link` mode resolves every symbol and exercises the host-only entry
     points; the known-answer run on a GPU is tests/test_gpu_loss_op.py::test_abi_harness_kat."""
     import subprocess
@@ -96,8 +96,6 @@ def test_reference_header_links_against_this_library():
     from rnnt_speech_recognition_b200 import _lib
     _lib.load()
     exe = ge.build_abi_harness()
-    if exe is None:
-        pytest.skip("no /root/reference here and no prebuilt harness")
     r = subprocess.run([exe, "link"], capture_output=True, text=True, timeout=60)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "link ok" in r.stdout

@@ -4,7 +4,7 @@ is present in this container, the unmodified reference library itself (oracle/_r
 import numpy as np
 import pytest
 
-from conftest import assert_close, fp32_tol, golden_names, load
+from conftest import GOLDEN, assert_close, fp32_tol, golden_names, load
 
 
 def softmax_chain(lp_grads, log_probs):
@@ -107,25 +107,32 @@ def test_numeric_gradient(oracle):
     assert rel < 1e-8
 
 
+def ref_cases():
+    """Outputs of the unmodified reference library for the inputs of tests/golden/make_ref_cases.py."""
+    import importlib.util
+    import os
+    spec = importlib.util.spec_from_file_location("make_ref_cases", os.path.join(GOLDEN, "make_ref_cases.py"))
+    mrc = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mrc)
+    return mrc, load("ref_cases.npz")
+
+
 def test_against_live_reference(oracle):
-    """When the unmodified reference library is available (this container, or shipped to the GPU
-    box in oracle/_ref) the restatement must agree with it on fresh random input."""
-    if not oracle.have_ref():
-        pytest.skip("oracle/_ref/libwarprnnt.so not available")
-    rng = np.random.default_rng(99)
-    B, T, U, V = 4, 13, 6, 9
-    acts = rng.standard_normal((B, T, U, V)).astype(np.float32)
-    labels = rng.integers(1, V, (B, U - 1)).astype(np.int32)
-    il = np.array([13, 7, 1, 10], np.int32)
-    ll = np.array([5, 2, 0, 4], np.int32)
-    lp = oracle.log_softmax(acts)
+    """The restatement agrees with the unmodified reference library on random input: live when oracle/_ref is built,
+    otherwise against the reference's stored outputs (tests/golden/ref_cases.npz)."""
+    mrc, gold = ref_cases()
+    lp, labels, il, ll = mrc.live_case(oracle)
     c, g = oracle.rnnt_cost_and_grad(lp, labels, il, ll)
-    cr, gr = oracle.ref_cpu_cost_and_grad(lp, labels, il, ll, num_threads=2)
+    cr, gr, ws = gold["live_costs"], gold["live_grads"], int(gold["live_ws_gpu"])
+    if oracle.have_ref():
+        cr, gr = oracle.ref_cpu_cost_and_grad(lp, labels, il, ll, num_threads=2)
+        import ctypes as C
+        s = C.c_size_t(0)
+        assert oracle.ref().get_workspace_size(13, 6, 4, True, C.byref(s), 4) == 0
+        ws = s.value
     assert np.allclose(c, cr, rtol=1e-6) and np.allclose(g, gr, rtol=1e-5, atol=1e-7)
-    rc, sz = oracle.get_workspace_size(T, U, B, True)
-    import ctypes as C
-    s = C.c_size_t(0)
-    assert oracle.ref().get_workspace_size(T, U, B, True, C.byref(s), 4) == rc == 0 and s.value == sz
+    rc, sz = oracle.get_workspace_size(13, 6, 4, True)
+    assert rc == 0 and ws == sz
 
 
 def test_invalid_arguments(oracle):
@@ -135,52 +142,35 @@ def test_invalid_arguments(oracle):
 
 
 def test_against_live_reference_property(oracle):
-    """Property-based pin (hypothesis, fixed seed database off): on random shapes, ragged lengths, blank positions and
-    logit scales the restatement and the unmodified reference library agree on costs and log-prob gradients."""
-    if not oracle.have_ref():
-        pytest.skip("oracle/_ref/libwarprnnt.so not available")
-    from hypothesis import given, settings, strategies as st, HealthCheck
-
-    @settings(max_examples=40, deadline=None, derandomize=True, database=None,
-              suppress_health_check=[HealthCheck.too_slow, HealthCheck.data_too_large])
-    @given(st.integers(1, 4), st.integers(1, 12), st.integers(1, 7), st.integers(2, 11), st.integers(0, 2 ** 31 - 1),
-           st.sampled_from([0.3, 1.0, 6.0]))
-    def run(B, T, U, V, seed, scale):
-        rng = np.random.default_rng(seed)
-        acts = (scale * rng.standard_normal((B, T, U, V))).astype(np.float32)
-        blank = int(rng.integers(0, V))
-        cand = np.array([v for v in range(V) if v != blank])
-        labels = (rng.choice(cand, size=(B, U - 1)).astype(np.int32) if U > 1 else np.zeros((B, 0), np.int32))
-        il = rng.integers(1, T + 1, B).astype(np.int32)
-        ll = rng.integers(0, U, B).astype(np.int32)
-        il[0], ll[0] = T, U - 1                       # the reference sizes its slabs by maxT / maxU
-        lp = oracle.log_softmax(acts)
+    """On random shapes, ragged lengths, blank positions and logit scales (a fixed sequence of cases) the restatement and
+    the unmodified reference library agree on costs and log-prob gradients (live, or its stored outputs)."""
+    mrc, gold = ref_cases()
+    for i in range(mrc.N_CPU_CASES):
+        lp, labels, il, ll, blank = mrc.cpu_case(oracle, i)
         c, g = oracle.rnnt_cost_and_grad(lp, labels, il, ll, blank=blank)
-        cr, gr = oracle.ref_cpu_cost_and_grad(lp, labels, il, ll, blank=blank, num_threads=1)
-        assert np.allclose(c, cr, rtol=1e-5, atol=1e-6), (B, T, U, V, seed)
-        assert np.allclose(g, gr, rtol=1e-4, atol=1e-6), (B, T, U, V, seed)
-
-    run()
+        if oracle.have_ref():
+            cr, gr = oracle.ref_cpu_cost_and_grad(lp, labels, il, ll, blank=blank, num_threads=1)
+        else:
+            cr, gr = gold["cpu%d_costs" % i], gold["cpu%d_grads" % i]
+        assert np.allclose(c, cr, rtol=1e-5, atol=1e-6), (i, lp.shape)
+        assert np.allclose(g, gr, rtol=1e-4, atol=1e-6), (i, lp.shape)
 
 
 def test_joint_oracle_against_torch_fp64_chain_property(oracle):
     """The joint is parity-unpinned by the reference (TensorFlow arithmetic): its anchor is model.py:158-166 restated in
     torch fp64 and chained by autograd through log_softmax into the reference library's fp64 entry point
-    (tests/golden/make_golden.py: joint_case).  Fresh random shapes here, beyond the committed fixtures."""
-    if not oracle.have_ref():
-        pytest.skip("oracle/_ref/libwarprnnt.so not available")
-    import importlib.util
-    import os
-    spec = importlib.util.spec_from_file_location("make_golden", os.path.join(os.path.dirname(__file__), "golden", "make_golden.py"))
-    mg = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mg)
-    rng = np.random.default_rng(20260924)
-    for _ in range(10):
-        B, T, U = int(rng.integers(1, 4)), int(rng.integers(1, 9)), int(rng.integers(1, 6))
-        V, H = int(rng.integers(2, 9)), int(rng.integers(1, 7))
-        k = mg.joint_case(rng, B, T, U, V, H, blank=int(rng.integers(0, V)), ragged=bool(rng.integers(0, 2)))
+    (tests/golden/make_golden.py: joint_case).  Ten random shapes beyond the committed fixtures: generated live when
+    oracle/_ref is built, otherwise the stored chain results."""
+    mrc, gold = ref_cases()
+    if oracle.have_ref():
+        cases = mrc.joint_cases()
+    else:
+        cases = [{n[len("joint%d_" % i):]: gold[n] for n in gold if n.startswith("joint%d_" % i)}
+                 for i in range(mrc.N_JOINT_CASES)]
+    for k in cases:
+        B = k["enc"].shape[0]
         o64 = oracle.joint_loss_grad(*(k[n].astype(np.float64) for n in ("enc", "pred", "W", "b")), k["labels"],
                                      k["input_lengths"], k["label_lengths"], int(k["blank"]), grad_scale=np.full(B, 1.0 / B))
-        assert np.allclose(o64["costs"], k["costs"], rtol=1e-10), (B, T, U, V, H)
+        assert np.allclose(o64["costs"], k["costs"], rtol=1e-10), k["enc"].shape
         for g in ("d_enc", "d_pred", "dW", "db"):
-            assert np.allclose(o64[g], k[g], rtol=1e-9, atol=1e-11), (g, B, T, U, V, H)
+            assert np.allclose(o64[g], k[g], rtol=1e-9, atol=1e-11), (g, k["enc"].shape)

@@ -1,5 +1,5 @@
-"""Materialised-logits op (compute_rnnt_loss drop-in) on one B200: this library vs the reference's own SIMT CUDA
-kernels (warp-transducer compiled unmodified for sm_100 into oracle/_ref/libwarprnnt_gpu.so).
+"""Materialised-logits op (compute_rnnt_loss drop-in) on one H100: this library vs the reference's own SIMT CUDA
+kernels (warp-transducer compiled unmodified for sm_90 into oracle/_ref/libwarprnnt_gpu.so).
 
   python tools/bench_op.py [B T U V]      default BASELINE C2 (16 256 64 256) and a larger (32 512 128 1024) case
 
@@ -72,7 +72,7 @@ def run_shapes(shapes):
             g2 = torch.empty_like(x)
             c2 = np.zeros(B, np.float32)
             ms2 = run_lib(R, "compute_rnnt_loss", x, g2, lab, il, ll, ws2, c2, _lib.RnntOptions)
-            res["reference_simt_sm100"] = {"ms": ms2, "GBps": byts / ms2 / 1e6}
+            res["reference_simt_sm90"] = {"ms": ms2, "GBps": byts / ms2 / 1e6}
             res["max_abs_grad_diff"] = (g1 - g2).abs().max().item()
             res["max_rel_cost_diff"] = float(np.abs(c1 - c2).max() / np.abs(c2).max())
             res["speedup"] = ms2 / ms
