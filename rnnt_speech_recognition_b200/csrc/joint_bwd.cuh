@@ -10,10 +10,10 @@
 //                   a run of tiles and stored once) and over t (-> one fp32 partial plane of d_pred per t-block).
 //                   Neither dl nor dZ ever exists in HBM.
 //   bwd_dw_kernel   [dW; db][H+1,V] (+)= ([rs_row * z, rs_row])^T . E'  as a split-K GEMM over the lattice rows: the A operand
-//                   is REGENERATED from enc/pred by the consumer warpgroups themselves (tanh, times the row scale, K-major
-//                   SWIZZLE_128B) while the previous K step's MMAs run; row H of A is the row scale itself, so row H of the
-//                   product is db = sum_rows dl.  The B operand is E' loaded MN-major by TMA.  Partial tiles go to fp32
-//                   planes (deterministic), summed by sum_planes_kernel.
+//                   is REGENERATED from enc/pred (tanh, times the row scale, K-major SWIZZLE_128B) by a producer warpgroup
+//                   into a ring ahead of the two MMA warpgroups, from inputs TMA brought into shared memory a slot ahead;
+//                   row H of A is the row scale itself, so row H of the product is db = sum_rows dl.  The B operand is E'
+//                   loaded MN-major by TMA.  Partial tiles go to fp32 planes (deterministic), summed by sum_planes_kernel.
 //
 // All operands bf16 (E' needs the exponent range: it is relative to a reference that may lie far below the row maximum),
 // fp32 accumulation.  Tile geometry: 16 x 8 lattice tiles (TT = 16 time steps, UU = 8 label positions), row r = tl*8 + ul;
@@ -24,12 +24,12 @@
 namespace rb {
 
 constexpr int BW_TT = 16, BW_UU = 8;
-constexpr int BWD_THREADS = 288;        // warps 0-3 / 4-7: consumer warpgroups (M = 64 each) | warp 8: TMA
+constexpr int BWD_THREADS = 288;        // dZ: warps 0-3 / 4-7: consumer warpgroups (M = 64 each) | warp 8: TMA
 constexpr int DZ_NC = 128;              // h columns per dZ pass (m64n128 accumulators)
 constexpr int DZ_GS_LD = DZ_NC + 8;     // row stride (floats) of the staged gradient tile
 constexpr int DZ_MAX_STAGES = 4;
 constexpr int DW_NV = 128;              // vocabulary columns per dW output tile
-constexpr int DW_STAGES = 4;
+constexpr int DW_STAGES = 4;            // K steps in flight between the producers and the MMA warpgroups (A + B per stage)
 
 struct BwdParams {
     const float* enc; const float* pred;
@@ -233,8 +233,22 @@ __global__ void __launch_bounds__(256) sum_pred_planes_kernel(const float4* __re
 // dW kernel
 // ---------------------------------------------------------------------------------------------------------------
 // CTA = (v-tile of DW_NV columns, 128-row block of [dW rows 0..H-1, db], split of the lattice rows).  K step = half a tile
-// (64 lattice rows: 8 time steps x 8 label positions).  Each consumer warpgroup owns 64 rows of the block and produces
-// their A tile [64 h x 64 k] (double-buffered) while the previous step's MMAs run.
+// (64 lattice rows: 8 time steps x 8 label positions).  Warp-specialised:
+//   warps 0-7    two consumer warpgroups (64 rows of the block each): wait for a stage, 4 x wgmma m64n128k16, release it
+//   warps 8-15   two producer warpgroups: build A [128 h x 64 k] = bf16(rs_row * tanh(enc + pred)) for both consumers from
+//                the slot's inputs in shared memory; thread = one A row, producer warpgroup = 4 of a K step's 8 time rows.
+//                Each SM sub-partition holds two producer warps, so the tanh work uses every MUFU unit and one warp's
+//                shared-memory latency is hidden behind the other's arithmetic (with a single producer warp per
+//                sub-partition the kernel was about 14 % slower at C3).
+//   warp 16      TMA: per slot the enc [16 x 128 h] / pred [8 x 128 h] fp32 boxes, the 128 row scales and the slot's meta
+//                into the input ring one slot ahead; per K step the E' boxes [64 k x 128 v] into the stage ring.
+// A stage holds A and B of one K step; its full barrier completes with the TMA bytes and one arrival per producer warp.
+// A warpgroup whose 64 rows all lie past row H (the second half of the db-only block when H % 128 == 0) does nothing.
+constexpr int DW_PWG = 2;                                   // producer warpgroups
+constexpr int DW_TMA_WARP = 8 + 4 * DW_PWG, DW_THREADS = 32 * (DW_TMA_WARP + 1);
+constexpr int DW_TL = 8 / DW_PWG;                           // time rows of a K step per producer thread
+constexpr int DW_IN_STAGES = 3;
+constexpr int DW_IN_ENC = 0, DW_IN_PRED = 8192, DW_IN_RS = 12288, DW_IN_META = 12800, DW_IN_BYTES = 13312;
 struct DwWork { int vt, hb, split; };
 __device__ __forceinline__ DwWork dw_decode(const BwdParams& p, int cta) {
     DwWork w;
@@ -246,36 +260,57 @@ __device__ __forceinline__ DwWork dw_decode(const BwdParams& p, int cta) {
     return w;
 }
 
-__global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dw_kernel(const __grid_constant__ CUtensorMap tmap_e, const BwdParams p) {
+__global__ void __launch_bounds__(DW_THREADS, 1) bwd_dw_kernel(const __grid_constant__ CUtensorMap tmap_e,
+                                                               const __grid_constant__ CUtensorMap tmap_enc,
+                                                               const __grid_constant__ CUtensorMap tmap_pred, const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    // B stages: [64 k x 128 v] as two [64 k x 64 v] boxes (MN-major, SW128) | A: [warpgroup][buffer][64 h x 64 k] K-major
+    // stage st: B = E' [64 k x 128 v] as two [64 k x 64 v] boxes (MN-major, SW128) at bsm + st * 16384 | A [128 h x 64 k]
+    // K-major SW128 at asm_ + st * 16384 (rows 0-63: consumer 0, rows 64-127: consumer 1) | input ring | barriers
     uint8_t* bsm = smem;
     uint8_t* asm_ = smem + DW_STAGES * 16384;
-    uint64_t* full = reinterpret_cast<uint64_t*>(asm_ + 4 * 8192);
+    uint8_t* ism = asm_ + DW_STAGES * 16384;
+    uint64_t* full = reinterpret_cast<uint64_t*>(ism + DW_IN_STAGES * DW_IN_BYTES);
     uint64_t* empty = full + DW_STAGES;
+    uint64_t* in_full = empty + DW_STAGES;
+    uint64_t* in_empty = in_full + DW_IN_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const DwWork wk = dw_decode(p, blockIdx.x);
-    const int v0 = wk.vt * DW_NV, nbox = min(DW_NV, p.V - v0) >> 6;
+    const int v0 = wk.vt * DW_NV, nbox = min(DW_NV, p.V - v0) >> 6, h0 = wk.hb * 128;
+    const int nwg = h0 + 64 > p.H ? 1 : 2;                             // consumer warpgroups with a row <= H
     if (threadIdx.x == 0) {
-        for (int i = 0; i < DW_STAGES; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 2); }
+        for (int i = 0; i < DW_STAGES; ++i) { ptx::mbar_init(&full[i], 1 + 2 * DW_PWG * nwg); ptx::mbar_init(&empty[i], nwg); }
+        for (int i = 0; i < DW_IN_STAGES; ++i) { ptx::mbar_init(&in_full[i], 1); ptx::mbar_init(&in_empty[i], 2 * DW_PWG * nwg); }
         ptx::fence_barrier_init();
     }
     if (nbox == 1)      // a 64-wide last v-tile: the second box of every stage is never loaded and reads as zeros
-        for (int i = threadIdx.x; i < DW_STAGES * 512; i += BWD_THREADS)
+        for (int i = threadIdx.x; i < DW_STAGES * 512; i += DW_THREADS)
             reinterpret_cast<uint4*>(bsm + (size_t)(i >> 9) * 16384 + 8192)[i & 511] = make_uint4(0u, 0u, 0u, 0u);
     ptx::fence_proxy_async_smem();
-    if (warp == 8 && lane == 0) ptx::prefetch_tmap(&tmap_e);
+    if (warp == DW_TMA_WARP && lane == 0) { ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_enc); ptx::prefetch_tmap(&tmap_pred); }
     __syncthreads();
     const long long cnt = *p.count;
     const int s_beg = (int)(cnt * wk.split / p.S), s_end = (int)(cnt * (wk.split + 1) / p.S);
 
-    if (warp == 8) {
-        // ===================== TMA: B = kept numerators, boxes [64 rows x 64 v] (rows = K) =====================
+    if (warp == DW_TMA_WARP) {
+        // ===================== TMA: the producer's inputs per slot, B = kept numerators per K step =====================
         if (lane == 0) {
-            int st = 0; uint32_t ph = 0;
-            for (int s = s_beg; s < s_end; ++s)
+            int st = 0, is = 0; uint32_t ph = 0, iph = 0;
+            auto load_inputs = [&](int s) {
+                ptx::mbar_wait(&in_empty[is], iph ^ 1);
+                uint8_t* in = ism + (size_t)is * DW_IN_BYTES;
+                const int4 m = __ldg(p.slot_meta + s);
+                ptx::sts128(ptx::smem_u32(in + DW_IN_META), make_uint4((uint32_t)m.x, (uint32_t)m.y, (uint32_t)m.z, (uint32_t)m.w));
+                ptx::mbar_arrive_expect_tx(&in_full[is], (uint32_t)(DW_IN_META - DW_IN_ENC));
+                ptx::tma_load_2d(in + DW_IN_ENC, &tmap_enc, &in_full[is], h0, m.x);
+                ptx::tma_load_2d(in + DW_IN_PRED, &tmap_pred, &in_full[is], h0, m.y);
+                ptx::bulk_load_1d(in + DW_IN_RS, p.rowscale + (size_t)s * 128, 512u, &in_full[is]);
+                if (++is == DW_IN_STAGES) { is = 0; iph ^= 1; }
+            };
+            if (s_beg < s_end) load_inputs(s_beg);
+            for (int s = s_beg; s < s_end; ++s) {
+                if (s + 1 < s_end) load_inputs(s + 1);
                 for (int half = 0; half < 2; ++half) {
                     ptx::mbar_wait(&empty[st], ph ^ 1);
                     ptx::mbar_arrive_expect_tx(&full[st], (uint32_t)nbox * 8192u);
@@ -283,69 +318,90 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dw_kernel(const __grid_con
                         ptx::tma_load_2d(bsm + (size_t)st * 16384 + j * 8192, &tmap_e, &full[st], v0 + 64 * j, s * 128 + half * 64);
                     if (++st == DW_STAGES) { st = 0; ph ^= 1; }
                 }
+            }
         }
         return;
     }
 
-    // ===================== consumer warpgroups: produce A, D[64 h x 128 v] += A[64 h x 64 k] . E'[64 k x 128 v] =====================
-    const int wg = threadIdx.x >> 7, t128 = threadIdx.x & 127, q = lane & 3;
-    const int hl = t128 & 63, hq = t128 >> 6;                         // A row of this thread; which 4 of a K step's 8 time rows
-    const int h = wk.hb * 128 + wg * 64 + hl;
-    const int kind = h < p.H ? 0 : (h == p.H ? 1 : 2);                // z row | row-scale row (db) | zero row
-    const int hc = min(h, p.H - 1);
-    const uint32_t a_a = ptx::smem_u32(asm_) + (uint32_t)wg * 16384u, b_a = ptx::smem_u32(bsm);
+    if (warp >= 8) {
+        // ===================== producers: A row `row`, time rows [tl0, tl0 + DW_TL) of every K step =====================
+        const int row = (threadIdx.x - 256) & 127, tl0 = ((threadIdx.x - 256) >> 7) * DW_TL, h = h0 + row;
+        if (h0 + (row >> 6) * 64 > p.H) return;                        // rows of an idle consumer warpgroup
+        const int kind = h < p.H ? 0 : (h == p.H ? 1 : 2);              // z row | row-scale row (db) | zero row
+        const uint32_t a_a = ptx::smem_u32(asm_) + (uint32_t)row * 128u, i_a = ptx::smem_u32(ism);
+        int st = 0, is = 0; uint32_t ph = 0, iph = 0;
+        for (int s = s_beg; s < s_end; ++s) {
+            ptx::mbar_wait_warp(&in_full[is], iph);
+            const uint32_t in = i_a + (uint32_t)is * DW_IN_BYTES;
+            // 8 pred rows and 16 enc rows of column h; rows past the padded arrays are clamped (their row scale is 0)
+            const uint4 m = ptx::lds128(in + DW_IN_META);
+            float pv[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) pv[k] = __uint_as_float(ptx::lds32(in + DW_IN_PRED + (uint32_t)(min(k, (int)m.w - 1) * 128 + row) * 4u));
+            for (int half = 0; half < 2; ++half) {
+                // every shared load of the half is issued before the first tanh: the accesses are volatile, so they keep
+                // source order, and with one or two producer warps per sub-partition nothing else hides their latency
+                float ev[DW_TL];
+                float4 rs4[2 * DW_TL];
+#pragma unroll
+                for (int j = 0; j < DW_TL; ++j)
+                    ev[j] = __uint_as_float(ptx::lds32(in + DW_IN_ENC + (uint32_t)(min(half * 8 + tl0 + j, (int)m.z - 1) * 128 + row) * 4u));
+#pragma unroll
+                for (int j = 0; j < 2 * DW_TL; ++j) rs4[j] = ptx::lds128f(in + DW_IN_RS + (uint32_t)(half * 64 + tl0 * 8 + 4 * j) * 4u);
+                ptx::mbar_wait_warp(&empty[st], ph ^ 1);
+                const uint32_t abuf = a_a + (uint32_t)st * 16384u;
+#pragma unroll
+                for (int j = 0; j < DW_TL; ++j) {
+                    const int tl = tl0 + j;
+                    const float rsv[8] = {rs4[2 * j].x, rs4[2 * j].y, rs4[2 * j].z, rs4[2 * j].w,
+                                          rs4[2 * j + 1].x, rs4[2 * j + 1].y, rs4[2 * j + 1].z, rs4[2 * j + 1].w};
+                    float z[8];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k)
+                        z[k] = kind == 0 ? ptx::tanh_approx(ev[j] + pv[k]) * rsv[k] : (kind == 1 ? rsv[k] : 0.f);
+                    ptx::sts128(abuf + (uint32_t)((tl ^ (row & 7)) << 4),
+                                make_uint4(ptx::pack_bf16x2(z[0], z[1]), ptx::pack_bf16x2(z[2], z[3]), ptx::pack_bf16x2(z[4], z[5]),
+                                           ptx::pack_bf16x2(z[6], z[7])));
+                }
+                ptx::fence_proxy_async_smem();
+                __syncwarp();
+                if (lane == 0) ptx::mbar_arrive(&full[st]);
+                if (++st == DW_STAGES) { st = 0; ph ^= 1; }
+            }
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&in_empty[is]);
+            if (++is == DW_IN_STAGES) { is = 0; iph ^= 1; }
+        }
+        return;
+    }
+
+    // ===================== consumer warpgroups: D[64 h x 128 v] += A[64 h x 64 k] . E'[64 k x 128 v] =====================
+    const int wg = warp >> 2, t128 = threadIdx.x & 127, q = lane & 3;
+    if (h0 + wg * 64 > p.H) return;
+    const uint32_t a_a = ptx::smem_u32(asm_) + (uint32_t)wg * 8192u, b_a = ptx::smem_u32(bsm);
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    int st = 0, prev = -1; uint32_t ph = 0, it = 0;
-    for (int s = s_beg; s < s_end; ++s) {
-        // this slot's inputs: 8 pred rows and 8 enc rows (4 per half) of column h; rows past the padded arrays are clamped
-        // (their row scale is 0)
-        const int4 m = __ldg(p.slot_meta + s);
-        float pv[8], ev[8];
-        if (kind == 0) {
+    int st = 0, prev = -1; uint32_t ph = 0;
+    for (int step = 2 * s_beg; step < 2 * s_end; ++step) {
+        ptx::mbar_wait_warp(&full[st], ph);
+        const uint64_t ad = ptx::gmma_desc_k_sw128(a_a + (uint32_t)st * 16384u), bd = ptx::gmma_desc_mn_sw128(b_a + (uint32_t)st * 16384u, 8192u);
+        ptx::wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 8; ++k) pv[k] = __ldg(p.pred + (size_t)(m.y + min(k, m.w - 1)) * p.H + hc);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) ev[k] = __ldg(p.enc + (size_t)(m.x + min((k >> 2) * 8 + hq * 4 + (k & 3), m.z - 1)) * p.H + hc);
-        }
-        for (int half = 0; half < 2; ++half, ++it) {
-            const uint32_t abuf = a_a + (it & 1) * 8192u;
-            const float* rsp = p.rowscale + (size_t)s * 128 + half * 64;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int tl = hq * 4 + j;
-                const float4 r0 = __ldg(reinterpret_cast<const float4*>(rsp + tl * 8)), r1 = __ldg(reinterpret_cast<const float4*>(rsp + tl * 8 + 4));
-                const float rsv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-                float z[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    z[k] = kind == 0 ? ptx::tanh_approx(ev[half * 4 + j] + pv[k]) * rsv[k] : (kind == 1 ? rsv[k] : 0.f);
-                ptx::sts128(abuf + (uint32_t)(hl * 128 + ((tl ^ (hl & 7)) << 4)),
-                            make_uint4(ptx::pack_bf16x2(z[0], z[1]), ptx::pack_bf16x2(z[2], z[3]), ptx::pack_bf16x2(z[4], z[5]),
-                                       ptx::pack_bf16x2(z[6], z[7])));
-            }
-            ptx::fence_proxy_async_smem();
-            ptx::named_bar_sync(1 + wg, 128);
-            ptx::mbar_wait(&full[st], ph);
-            const uint64_t ad = ptx::gmma_desc_k_sw128(abuf), bd = ptx::gmma_desc_mn_sw128(b_a + (uint32_t)st * 16384u, 8192u);
-            ptx::wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k)   // K = 16 lattice rows per MMA: 32 B along A's rows, 16 x 128 B of B
-                ptx::wgmma_m64n128_bf16<1>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 128), 1u);
-            ptx::wgmma_commit();
-            ptx::wgmma_wait<1>();        // the previous step's MMAs have retired: its B stage and A buffer are free
-            if (prev >= 0 && t128 == 0) ptx::mbar_arrive(&empty[prev]);
-            prev = st;
-            if (++st == DW_STAGES) { st = 0; ph ^= 1; }
-        }
+        for (int k = 0; k < 4; ++k)   // K = 16 lattice rows per MMA: 32 B along A's rows, 16 x 128 B of B
+            ptx::wgmma_m64n128_bf16<1>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 128), 1u);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<1>();        // the previous step's MMAs have retired: its stage is free
+        if (prev >= 0 && t128 == 0) ptx::mbar_arrive(&empty[prev]);
+        prev = st;
+        if (++st == DW_STAGES) { st = 0; ph ^= 1; }
     }
     ptx::wgmma_wait<0>();
     if (prev >= 0 && t128 == 0) ptx::mbar_arrive(&empty[prev]);
     ptx::fence_regs(acc);
     if (s_end <= s_beg) return;
     // ---- epilogue: rows (Ra, Ra + 8) x 32 columns of the block -> accumulated into the split's partial plane
-    const int Ra = wk.hb * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int Ra = h0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
     for (int ri = 0; ri < 2; ++ri) {
         const int hr = Ra + 8 * ri;
@@ -373,7 +429,7 @@ inline DwGeom dw_geometry(int H, int V) {
     g.S = 4 * TC_SMS / (g.nVT * g.nHB);
     if (g.S < 1) g.S = 1;
     if (g.S > 64) g.S = 64;
-    g.smem_bytes = 1024 + (size_t)DW_STAGES * 16384 + 4 * 8192 + 2 * DW_STAGES * 8;
+    g.smem_bytes = 1024 + (size_t)DW_STAGES * 32768 + (size_t)DW_IN_STAGES * DW_IN_BYTES + 2 * (DW_STAGES + DW_IN_STAGES) * 8;
     return g;
 }
 

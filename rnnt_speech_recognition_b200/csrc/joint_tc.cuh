@@ -202,6 +202,18 @@ inline bool make_tmap_bf16(CUtensorMap* tm, const void* base, uint64_t rows, uin
               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+// 2-D row-major fp32 matrix [rows x cols], box [box_rows x 128 cols] stored densely (no swizzle); out-of-range reads as 0
+inline bool make_tmap_f32(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    PFN_encodeTiled fn = get_encode_fn();
+    if (!fn) return false;
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {cols * 4};
+    cuuint32_t box[2] = {128, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr,
+              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 // Workspace of the tensor-core path (a pure function of the descriptor).  The kept arrays (numerators + maxima) are
 // laid out per 128-row tile; the batch is processed in utterance chunks that keep them under ~16 GiB.
@@ -378,9 +390,10 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
     if (cudaMemsetAsync(sc.dWp, 0, sizeof(float) * (size_t)wg.S * d.H * d.V, s) != cudaSuccess ||
         cudaMemsetAsync(sc.dbp, 0, sizeof(float) * (size_t)wg.S * d.V, s) != cudaSuccess)
         return RNNT_STATUS_MEMOPS_FAILED;
-    CUtensorMap tm_e128, tm_e64, tm_w;
+    CUtensorMap tm_e128, tm_e64, tm_w, tm_enc, tm_pred;
     if (!make_tmap_bf16(&tm_e128, sc.dl, sc.rows_chunk, d.V, 128) || !make_tmap_bf16(&tm_e64, sc.dl, sc.rows_chunk, d.V, 64) ||
-        !make_tmap_bf16(&tm_w, sc.Wb, d.H, d.V, DZ_NC)) {
+        !make_tmap_bf16(&tm_w, sc.Wb, d.H, d.V, DZ_NC) ||
+        !make_tmap_f32(&tm_enc, enc, (uint64_t)d.B * d.maxT, d.H, BW_TT) || !make_tmap_f32(&tm_pred, pred, (uint64_t)d.B * d.maxU, d.H, BW_UU)) {
         fprintf(stderr, "rnnt_b200: cuTensorMapEncodeTiled failed\n");
         return RNNT_STATUS_EXECUTION_FAILED;
     }
@@ -422,7 +435,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         }
         {
             ScopedTimer tmr("bwd_dw_kernel", s);
-            bwd_dw_kernel<<<wg.nVT * wg.nHB * wg.S, BWD_THREADS, wg.smem_bytes, s>>>(tm_e64, p);
+            bwd_dw_kernel<<<wg.nVT * wg.nHB * wg.S, DW_THREADS, wg.smem_bytes, s>>>(tm_e64, tm_enc, tm_pred, p);
         }
         *launches += 3;
         if (cudaGetLastError() != cudaSuccess) return RNNT_STATUS_EXECUTION_FAILED;
