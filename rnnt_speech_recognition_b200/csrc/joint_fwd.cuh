@@ -15,10 +15,13 @@
 // MODE 0  forward: lse + (blank, label) log-probs per cell; nothing else leaves the SM
 // MODE 2  forward that KEEPS its activations (rnntb200JointDesc.keep_activations, and the backward's per-chunk
 //         recompute): MODE 0 + the softmax numerators E[row, v] = 2^(y_v - ref_row) as bf16, all columns of a row against
-//         ONE reference ref_row = the maximum of the row's first 32 logits (bf16 keeps its 8 significant bits over the whole
-//         exponent range, so any reference works; the exponent is clamped at +100), and ref_row itself.  The logit
-//         gradients are then row_scale * E: the two backward GEMMs take E straight from TMA.
-//         Both modes form the softmax sum with the same arithmetic, so they give identical costs.
+//         ONE reference ref_row, and ref_row itself.  ref_row starts as the maximum of the row's first 32 logits; a chunk
+//         holding a logit more than 2^FWD_REBASE above it raises it by whole octaves to at least that chunk's maximum
+//         (rescaling the numerators already stored), so every stored numerator is at most 2^FWD_REBASE and the row
+//         maximum is at most ref_row + FWD_REBASE.  bf16 keeps its 8 significant bits over the whole exponent range, so
+//         any reference in that window works.  The logit gradients are then row_scale * E: the two backward GEMMs take E
+//         straight from TMA.
+//         Both modes form the softmax sum and the reference with the same arithmetic, so they give identical costs.
 #pragma once
 #include <cuda_fp16.h>
 #include "joint_tc.cuh"
@@ -28,6 +31,7 @@ namespace rb {
 constexpr int FWD_THREADS = 288;
 constexpr int FWD_NC = 64;              // vocabulary columns per chunk (one m64n64 accumulator per warpgroup)
 constexpr int FWD_MAX_STAGES = 8;
+constexpr float FWD_REBASE = 64.f;      // log2 units: largest stored numerator 2^64, row maximum <= ref_row + 64
 
 struct FwdGeom { int stages; size_t smem_bytes; bool ok; };
 inline FwdGeom fwd_geometry(int H, int V) {
@@ -41,6 +45,31 @@ inline FwdGeom fwd_geometry(int H, int V) {
     g.smem_bytes = fixed + (size_t)g.stages * 8192;
     g.ok = g.stages >= 2;
     return g;
+}
+
+// Rebase of one row's reference (MODE comment above), called by all 32 lanes of the warp when a chunk holds a logit more
+// than 2^FWD_REBASE above the reference of any of its rows.  The quad takes a new reference a whole number of octaves
+// above the old one, at least the chunk's row maximum, and (MODE 2) each lane scales the numerators it stored for the
+// row's earlier chunks by that power of two: it reads back its own stores.  Inlined behind a warp-uniform branch:
+// as a real call (__noinline__) the keeping forward took 0.3 ms (4 %) longer at BASELINE C3, on an H100 80GB HBM3 at
+// 700 W, although ordinary inputs never take the branch.
+template <int MODE>
+__device__ __forceinline__ float fwd_rebase(float gm, float ref, __nv_bfloat16* dl, long long row, int V, int q, int c) {
+    float qm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 1));
+    qm = fmaxf(qm, __shfl_xor_sync(0xffffffffu, qm, 2));
+    if (!(qm - ref > FWD_REBASE)) return ref;
+    const float sh = ceilf(qm - ref);
+    if (MODE == 2 && row >= 0) {
+        const float f = ldexpf(1.f, -(int)fminf(sh, 200.f));
+        uint32_t* w = reinterpret_cast<uint32_t*>(dl + row * V + 2 * q);
+        for (int cc = 0; cc < c; ++cc)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const uint32_t v = w[cc * (FWD_NC / 2) + 4 * j];
+                w[cc * (FWD_NC / 2) + 4 * j] = ptx::pack_bf16x2(__uint_as_float(v << 16) * f, __uint_as_float(v & 0xffff0000u) * f);
+            }
+    }
+    return ref + sh;
 }
 
 template <int MODE>
@@ -172,35 +201,28 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) joint_fwd_kernel(const __grid_
                 float gm = y[0];
 #pragma unroll
                 for (int i = 1; i < 16; ++i) gm = fmaxf(gm, y[i]);
+                if (__any_sync(0xffffffffu, gm - ref[ri] > FWD_REBASE))      // never taken on ordinary inputs
+                    ref[ri] = fwd_rebase<MODE>(gm, ref[ri], p.dl, has_slot ? (long long)(rowbase + Ra + 8 * ri) : -1LL, p.V, q, c);
                 const float mn = fmaxf(m2[ri], gm);
                 uint32_t o[8];
-                float a = 0.f;
-                if (gm - ref[ri] <= 100.f) {
-                    float accr = 0.f;
+                float accr = 0.f;
 #pragma unroll
-                    for (int i = 0; i < 16; i += 2) {
-                        const float e0 = ptx::ex2_approx(y[i] - ref[ri]), e1 = ptx::ex2_approx(y[i + 1] - ref[ri]);
-                        accr += e0 + e1;
-                        if (MODE == 2) o[i >> 1] = ptx::pack_bf16x2(e0, e1);
-                    }
-                    a = accr * ptx::ex2_approx(ref[ri] - mn);
-                } else {
-                    // a logit more than 2^100 above the reference (never seen outside adversarial inputs): the sum is taken
-                    // against the running maximum, the stored values are clamped at 2^100
-#pragma unroll
-                    for (int i = 0; i < 16; i += 2) {
-                        a += ptx::ex2_approx(y[i] - mn) + ptx::ex2_approx(y[i + 1] - mn);
-                        if (MODE == 2)
-                            o[i >> 1] = ptx::pack_bf16x2(ptx::ex2_approx(fminf(y[i] - ref[ri], 100.f)),
-                                                         ptx::ex2_approx(fminf(y[i + 1] - ref[ri], 100.f)));
-                    }
+                for (int i = 0; i < 16; i += 2) {
+                    const float e0 = ptx::ex2_approx(y[i] - ref[ri]), e1 = ptx::ex2_approx(y[i + 1] - ref[ri]);
+                    accr += e0 + e1;
+                    if (MODE == 2) o[i >> 1] = ptx::pack_bf16x2(e0, e1);
                 }
+                // y - ref <= FWD_REBASE here, so accr is finite.  A lane whose logits all lie more than 2^126 below the
+                // quad's reference has accr == 0 (ex2 flushes), and its share of the row sum is below 2^-126 of it:
+                // the clamp keeps that product 0 instead of 0 * inf.  The rounding is spelled out (a rounded product, then
+                // one fma) so that MODE 0 and MODE 2 cannot be contracted differently and keep identical sums.
+                const float a = __fmul_rn(accr, ptx::ex2_approx(fminf(ref[ri] - mn, 126.f)));
                 if (MODE == 2 && has_slot) {
                     uint32_t* dst = reinterpret_cast<uint32_t*>(p.dl + (rowbase + Ra + 8 * ri) * p.V + col0 + 2 * q);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) dst[4 * j] = o[j];
                 }
-                s[ri] = s[ri] * ptx::ex2_approx(m2[ri] - mn) + a;
+                s[ri] = fmaf(s[ri], ptx::ex2_approx(m2[ri] - mn), a);
                 m2[ri] = mn;
                 // the blank and label logits: held by one lane of the quad, at a column index known only at run time
                 const int db = p.blank - col0 - 2 * q, dlb = lab[ri] - col0 - 2 * q;

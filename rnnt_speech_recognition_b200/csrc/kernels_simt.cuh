@@ -413,9 +413,16 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
         float dlb = g * (expf(lpb[k] + occ) - sb), dll = g * (pl - sl_);
         if (has_label && lab == blank) { dlb -= g * sl_; dll = dlb; }    // degenerate: label == blank
         rs = g * exp2f(rowref[row] + (occ - lse[((long long)b * maxT + t) * maxU + u]) * 1.4426950408889634f);
-        // cells whose whole gradient row is below 1e-30 contribute nothing: treating them as exactly 0 keeps 1/rs finite
-        // (a denormal rs would make it +inf and the patched columns NaN)
-        if (!(fabsf(rs) > 1e-30f && fabsf(rs) < CUDART_INF_F)) rs = 0.f;
+        // rs is cut to 0 only where 1/rs stops being finite (a denormal rs would make it +inf and the patched columns NaN).
+        // The forward keeps lse2 - ref <= FWD_REBASE + log2 V, so a row cut here has |g| * e^occ < 2^-126 * 2^(64 + log2 V):
+        // at V = 4096 below 2^-50, against rows of up to |g|.  The patched columns dl / rs are at most 2^(lse2 - ref),
+        // i.e. 2^76 at V = 4096, whatever g is: far inside the bf16 range.
+        // A cell of occupancy below 2^-64 whose rs is below 1e-30 is treated as 0 as well: its whole gradient row is below
+        // 2^-64 |g|, far under the fp32 resolution of every sum it joins, and bwd_dz_kernel skips the epilogue of rows
+        // with rs == 0.  (A cut on rs alone would also drop rows that matter once g or 2^(ref - lse2) is small.)
+        const float ars = fabsf(rs);
+        if (!(ars >= 1.17549435e-38f && ars < CUDART_INF_F) || (ars < 1e-30f && occ < -64.f * 0.6931471805599453f))
+            rs = 0.f;                                                    // 1.17549435e-38 = FLT_MIN
         const float inv = rs != 0.f ? 1.f / rs : 0.f;
         unsigned short* e = E + row * (long long)V;
         e[blank] = __bfloat16_as_ushort(__float2bfloat16(dlb * inv));
