@@ -130,6 +130,35 @@ rnntStatus_t rnntb200_loss_device(const float* activations, float* gradients, co
                                   int alphabet_size, int minibatch, float* costs_device, void* workspace,
                                   rnntOptions options);
 
+/** Element type of 16-bit logits (mixed-precision training: fp16 / bf16 activations). */
+typedef enum {
+    RNNTB200_LOGITS_F16 = 0,  /**< IEEE binary16 */
+    RNNTB200_LOGITS_BF16 = 1  /**< bfloat16 */
+} rnntb200LogitType;
+
+/** rnntb200_loss_device on 16-bit logits, split into a forward and a backward call so that the gradient is formed
+ *  only when it is asked for, with the upstream gradient multiplied in before its one rounding to 16 bits (an fp16
+ *  gradient of an unscaled cost underflows; a loss-scaled one does not).
+ *  activations  device, raw logits (B,maxT,maxU,V) row-major of type logit_type, softmax done inside
+ *  costs_device device float (B): -log p(y|x) per utterance
+ *  workspace    device, get_workspace_size(maxT, maxU, B, true, &sz, 4) bytes: the fp32 planes of the loss op.  The
+ *               forward fills it; the backward reads it and must get it unchanged.
+ *  All arithmetic is fp32: each logit is converted exactly on load, each gradient rounded to nearest-even on store.
+ *  Stream-ordered, no allocation, no host synchronisation (CUDA-graph capturable).  Errors: NULL pointers,
+ *  non-positive sizes, maxU > 1024, a blank outside [0, V) or an unknown logit_type -> RNNT_STATUS_INVALID_VALUE. */
+rnntStatus_t rnntb200_loss16_forward(const void* activations, int logit_type, const int* flat_labels,
+                                     const int* label_lengths, const int* input_lengths, int alphabet_size, int minibatch,
+                                     float* costs_device, void* workspace, rnntOptions options);
+
+/** Backward of rnntb200_loss16_forward (same activations, labels, lengths, options and workspace):
+ *  gradients (B,maxT,maxU,V) of type logit_type, device, OVERWRITTEN = grad_costs[b] * d(costs[b])/d(activations) in
+ *  one pass; padded cells are written 0.  grad_costs: optional DEVICE float (B), NULL means 1 (as grad_scale of
+ *  rnntb200_loss_device). */
+rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, const int* flat_labels,
+                                      const int* label_lengths, const int* input_lengths, const float* grad_costs,
+                                      int alphabet_size, int minibatch, void* gradients, const void* workspace,
+                                      rnntOptions options);
+
 typedef enum {
     RNNTB200_FP32_EXACT = 0, /**< fp32 CUDA-core arithmetic; parity gate rtol 1e-4 (BASELINE C1/C2) */
     RNNTB200_BF16_TC = 1     /**< 16-bit operands on wgmma tensor cores, fp32 accumulate (BASELINE C3-C5): the forward

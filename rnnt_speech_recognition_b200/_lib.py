@@ -11,6 +11,7 @@ SO = os.environ.get("RNNTB200_LIB") or os.path.join(HERE, "librnnt_b200.so")   #
 
 RNNT_CPU, RNNT_GPU = 0, 1
 FP32_EXACT, BF16_TC = 0, 1
+LOGITS_F16, LOGITS_BF16 = 0, 1
 
 
 class RnntOptions(C.Structure):
@@ -27,7 +28,8 @@ class JointDesc(C.Structure):
 
 
 EXPORTS = ("get_warprnnt_version", "rnntGetStatusString", "get_workspace_size", "compute_rnnt_loss",
-           "compute_rnnt_loss_fp64", "rnntb200_loss_device", "rnntb200_joint_workspace_size",
+           "compute_rnnt_loss_fp64", "rnntb200_loss_device", "rnntb200_loss16_forward", "rnntb200_loss16_backward",
+           "rnntb200_joint_workspace_size",
            "rnntb200_joint_loss_forward", "rnntb200_joint_loss_backward", "rnntb200_joint_logits", "rnntb200_joint_step",
            "rnntb200_dense1_forward", "rnntb200_dense1_backward",
            "rnntb200_launch_count", "rnntb200_build_info", "rnntb200_set_timing", "rnntb200_get_timing")
@@ -62,6 +64,8 @@ def load(build_if_missing=True):
     L.compute_rnnt_loss.argtypes = [vp, vp, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
     L.compute_rnnt_loss_fp64.argtypes = L.compute_rnnt_loss.argtypes
     L.rnntb200_loss_device.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
+    L.rnntb200_loss16_forward.argtypes = [vp, ci, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
+    L.rnntb200_loss16_backward.argtypes = [vp, ci, vp, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
     L.rnntb200_joint_workspace_size.argtypes = [C.POINTER(JointDesc), C.POINTER(C.c_size_t)]
     L.rnntb200_joint_loss_forward.argtypes = [C.POINTER(JointDesc)] + [vp] * 9
     L.rnntb200_joint_loss_backward.argtypes = [C.POINTER(JointDesc)] + [vp] * 13

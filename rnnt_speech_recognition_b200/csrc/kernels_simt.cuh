@@ -10,6 +10,7 @@
 //                       in the same pass (replaces the cudaMemsetAsync of gpu_rnnt.h:109)
 //   row_scale_kernel    per-row scales of the tensor-core backward GEMMs + the patch of the two special columns
 //   zgen/sgemm/...      fp32 building blocks of the exact (RNNTB200_FP32_EXACT) joint path
+// lse_gather and rnnt_grad also take fp16 / bf16 logits (and write gradients of that type) over fp32 arithmetic.
 //
 // Data layout ("skewed" planes): a per-utterance plane stores cell (t,u) at row n=t+u, column u:
 //     sk(b,t,u) = b*SK + (t+u)*maxU + u,   SK = (maxT+maxU-1)*maxU
@@ -17,6 +18,7 @@
 // (t*maxU+u) planes cannot offer (stride maxU-1 between neighbouring threads).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math_constants.h>
 #include <stdint.h>
@@ -58,6 +60,63 @@ __device__ __forceinline__ float log_sum_exp_fast(float a, float b) {
 __device__ __forceinline__ float  wave_lse(float a, float b)  { return log_sum_exp_fast(a, b); }
 __device__ __forceinline__ double wave_lse(double a, double b) { return log_sum_exp<double>(a, b); }
 
+// Element types of the loss op's logits and gradients (X) next to its workspace type (T = float or double).  A 16-bit
+// logit is widened exactly on load; a gradient is rounded to nearest-even once, on store.  For X == T both are no-ops.
+__device__ __forceinline__ float  widen(float x)         { return x; }
+__device__ __forceinline__ double widen(double x)        { return x; }
+__device__ __forceinline__ float  widen(__half x)        { return __half2float(x); }
+__device__ __forceinline__ float  widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+template <typename X, typename T> __device__ __forceinline__ X narrow(T v) { return v; }
+template <> __device__ __forceinline__ __half narrow<__half, float>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 narrow<__nv_bfloat16, float>(float v) { return __float2bfloat16_rn(v); }
+
+// 16 bytes of logits as the vectorised kernels move them: 4 fp32 or 8 fp16 / bf16 elements, widened to fp32 in registers.
+template <typename X> struct Vec16;
+template <> struct Vec16<float> {
+    static constexpr int N = 4, LOG2N = 2;
+    using Raw = float4;
+    __device__ static Raw neg_inf() { return make_float4(-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F); }
+    __device__ static void widen(const Raw& r, float (&f)[N]) { f[0] = r.x; f[1] = r.y; f[2] = r.z; f[3] = r.w; }
+    __device__ static Raw narrow(const float (&f)[N]) { return make_float4(f[0], f[1], f[2], f[3]); }
+};
+template <typename H2, typename X> struct Vec16Half {
+    static constexpr int N = 8, LOG2N = 3;
+    using Raw = uint4;
+    __device__ static void widen(const Raw& r, float (&f)[N]) {
+        const H2* h = reinterpret_cast<const H2*>(&r);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { f[2 * i] = rb::widen(h[i].x); f[2 * i + 1] = rb::widen(h[i].y); }
+    }
+    __device__ static Raw narrow(const float (&f)[N]) {
+        Raw r;
+        X* h = reinterpret_cast<X*>(&r);
+#pragma unroll
+        for (int i = 0; i < N; ++i) h[i] = rb::narrow<X, float>(f[i]);
+        return r;
+    }
+};
+template <> struct Vec16<__half> : Vec16Half<__half2, __half> {
+    __device__ static Raw neg_inf() { return make_uint4(0xfc00fc00u, 0xfc00fc00u, 0xfc00fc00u, 0xfc00fc00u); }
+};
+template <> struct Vec16<__nv_bfloat16> : Vec16Half<__nv_bfloat162, __nv_bfloat16> {
+    __device__ static Raw neg_inf() { return make_uint4(0xff80ff80u, 0xff80ff80u, 0xff80ff80u, 0xff80ff80u); }
+};
+
+// max of N values as a pairwise tree, and sum_i exp(f_i - m) added left to right (for N = 4 exactly the fp32 kernels'
+// fmaxf(fmaxf(x, y), fmaxf(z, w)) and expf(x - m) + expf(y - m) + expf(z - m) + expf(w - m))
+template <int N>
+__device__ __forceinline__ float tree_max(const float* f) {
+    if constexpr (N == 1) return f[0];
+    else return fmaxf(tree_max<N / 2>(f), tree_max<N / 2>(f + N / 2));
+}
+template <int N>
+__device__ __forceinline__ float sum_exp(const float (&f)[N], float m) {
+    float t = expf(f[0] - m);
+#pragma unroll
+    for (int i = 1; i < N; ++i) t += expf(f[i] - m);
+    return t;
+}
+
 template <typename T>
 __device__ __forceinline__ T warp_max(T v) {
 #pragma unroll
@@ -88,10 +147,11 @@ __device__ __forceinline__ long long sk_index(int b, int t, int u, int maxU, lon
 // lse + gather: one warp per lattice cell (row of V logits).  Row r of `logits` is natural cell
 // row0 + r.  Two in-cache passes (max, then sum exp(x-max)) reproduce the reference's
 // reduce_max / reduce_exp arithmetic; the row (<= 16 KB) is served by L1 on the second pass.
-// Writes lse[cell] (natural order) and lp_blank / lp_label at the skewed index.
+// Writes lse[cell] (natural order) and lp_blank / lp_label at the skewed index.  X: element type of the logits (T, or
+// fp16 / bf16 over a float workspace).
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) lse_gather_kernel(const T* __restrict__ logits, long long row0,
+template <typename T, typename X = T>
+__global__ void __launch_bounds__(256) lse_gather_kernel(const X* __restrict__ logits, long long row0,
                                                          long long nrows, int V, const int* __restrict__ xlen,
                                                          const int* __restrict__ ylen,
                                                          const int* __restrict__ labels, int maxT, int maxU,
@@ -104,32 +164,33 @@ __global__ void __launch_bounds__(256) lse_gather_kernel(const T* __restrict__ l
     const CellIdx c = decode_cell(cell, maxT, maxU);
     const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
     if (c.t >= Tn || c.u >= Un) return;  // padded cell: never read downstream
-    const T* x = logits + row * (long long)V;
+    const X* x = logits + row * (long long)V;
     T m = neg_inf<T>();
-    for (int v = lane; v < V; v += 32) { T xv = x[v]; m = xv > m ? xv : m; }
+    for (int v = lane; v < V; v += 32) { T xv = widen(x[v]); m = xv > m ? xv : m; }
     m = warp_max(m);
     T s = 0;
-    for (int v = lane; v < V; v += 32) s += xexp(x[v] - m);
+    for (int v = lane; v < V; v += 32) s += xexp(widen(x[v]) - m);
     s = warp_sum(s);
     if (lane == 0) {
         const T l = m + xlog(s);
         lse[cell] = l;
         const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
-        lpb[k] = x[blank] - l;
-        if (c.u < Un - 1) lpl[k] = x[labels[(long long)c.b * (maxU - 1) + c.u]] - l;
+        lpb[k] = widen(x[blank]) - l;
+        if (c.u < Un - 1) lpl[k] = widen(x[labels[(long long)c.b * (maxU - 1) + c.u]]) - l;
     }
 }
 
-// float4 fast path of lse_gather (V % 4 == 0, 16-byte aligned rows): each lane streams 16-byte pieces of the row;
-// rows of up to 1024 logits are held in registers between the max and the sum pass (ONE read of the logits),
-// longer rows take the second pass from L1/L2.
-template <int MAXV4>   // per-lane float4 capacity held in registers (8 -> V <= 1024); 0 -> always two passes
-__global__ void __launch_bounds__(256) lse_gather_vec_kernel(const float* __restrict__ logits, long long row0,
+// 16-byte fast path of lse_gather (V a multiple of Vec16<X>::N, 16-byte aligned rows): each lane streams 16-byte pieces
+// of the row; rows of up to MAXV * 32 pieces (fp32: 1024 logits, fp16 / bf16: 2048) are held in registers between the
+// max and the sum pass (ONE read of the logits), longer rows take the second pass from L1/L2.
+template <typename X, int MAXV>   // per-lane 16-byte pieces held in registers (8); 0 -> always two passes
+__global__ void __launch_bounds__(256) lse_gather_vec_kernel(const X* __restrict__ logits, long long row0,
                                                              long long nrows, int V, const int* __restrict__ xlen,
                                                              const int* __restrict__ ylen,
                                                              const int* __restrict__ labels, int maxT, int maxU,
                                                              long long SK, int blank, float* __restrict__ lse,
                                                              float* __restrict__ lpb, float* __restrict__ lpl) {
+    using P = Vec16<X>;
     const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
@@ -137,30 +198,38 @@ __global__ void __launch_bounds__(256) lse_gather_vec_kernel(const float* __rest
     const CellIdx c = decode_cell(cell, maxT, maxU);
     const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
     if (c.t >= Tn || c.u >= Un) return;
-    const float* x = logits + row * (long long)V;
-    const float4* x4 = reinterpret_cast<const float4*>(x);
-    const int n4 = V >> 2;
+    const X* x = logits + row * (long long)V;
+    const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
+    const int nv = V >> P::LOG2N;
     float m = -CUDART_INF_F, s = 0.f;
-    if (MAXV4 > 0 && n4 <= MAXV4 * 32) {
-        float4 r[MAXV4 > 0 ? MAXV4 : 1];
+    if (MAXV > 0 && nv <= MAXV * 32) {
+        typename P::Raw r[MAXV > 0 ? MAXV : 1];
 #pragma unroll
-        for (int i = 0; i < MAXV4; ++i) {
+        for (int i = 0; i < MAXV; ++i) {
             const int k = lane + 32 * i;
-            r[i] = (k < n4) ? __ldg(x4 + k) : make_float4(-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F);
-            m = fmaxf(m, fmaxf(fmaxf(r[i].x, r[i].y), fmaxf(r[i].z, r[i].w)));
+            r[i] = (k < nv) ? __ldg(xv + k) : P::neg_inf();
+            float f[P::N];
+            P::widen(r[i], f);
+            m = fmaxf(m, tree_max<P::N>(f));
         }
         m = warp_max(m);
 #pragma unroll
-        for (int i = 0; i < MAXV4; ++i) s += expf(r[i].x - m) + expf(r[i].y - m) + expf(r[i].z - m) + expf(r[i].w - m);
+        for (int i = 0; i < MAXV; ++i) {
+            float f[P::N];
+            P::widen(r[i], f);
+            s += sum_exp(f, m);
+        }
     } else {
-        for (int k = lane; k < n4; k += 32) {
-            const float4 v = __ldg(x4 + k);
-            m = fmaxf(m, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+        for (int k = lane; k < nv; k += 32) {
+            float f[P::N];
+            P::widen(__ldg(xv + k), f);
+            m = fmaxf(m, tree_max<P::N>(f));
         }
         m = warp_max(m);
-        for (int k = lane; k < n4; k += 32) {
-            const float4 v = __ldg(x4 + k);
-            s += expf(v.x - m) + expf(v.y - m) + expf(v.z - m) + expf(v.w - m);
+        for (int k = lane; k < nv; k += 32) {
+            float f[P::N];
+            P::widen(__ldg(xv + k), f);
+            s += sum_exp(f, m);
         }
     }
     s = warp_sum(s);
@@ -168,13 +237,15 @@ __global__ void __launch_bounds__(256) lse_gather_vec_kernel(const float* __rest
         const float l = m + logf(s);
         lse[cell] = l;
         const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
-        lpb[k] = x[blank] - l;
-        if (c.u < Un - 1) lpl[k] = x[labels[(long long)c.b * (maxU - 1) + c.u]] - l;
+        lpb[k] = widen(x[blank]) - l;
+        if (c.u < Un - 1) lpl[k] = widen(x[labels[(long long)c.b * (maxU - 1) + c.u]]) - l;
     }
 }
 
-// float4 fast path of rnnt_grad_kernel (same arithmetic, 16-byte loads/stores).
-__global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const float* logits, float* out, long long row0,
+// 16-byte fast path of rnnt_grad_kernel (same arithmetic, 16-byte loads/stores; fp16 / bf16 gradients are rounded once,
+// after the upstream gradient is multiplied in).
+template <typename X>
+__global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* out, long long row0,
                                                             long long nrows, int V, const int* __restrict__ xlen,
                                                             const int* __restrict__ ylen,
                                                             const int* __restrict__ labels, int maxT, int maxU,
@@ -183,18 +254,20 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const float* logits,
                                                             const float* __restrict__ betas,
                                                             const float* __restrict__ llf,
                                                             const float* __restrict__ gscale) {
+    using P = Vec16<X>;
     const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
     const long long cell = row0 + row;
     const CellIdx c = decode_cell(cell, maxT, maxU);
     const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
-    const float* x = logits + row * (long long)V;
-    const float4* x4 = reinterpret_cast<const float4*>(x);
-    float4* g4 = reinterpret_cast<float4*>(out + row * (long long)V);
-    const int n4 = V >> 2;
+    const X* x = logits + row * (long long)V;
+    const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
+    typename P::Raw* gv = reinterpret_cast<typename P::Raw*>(out + row * (long long)V);
+    const int nv = V >> P::LOG2N;
     if (c.t >= Tn || c.u >= Un) {
-        for (int k = lane; k < n4; k += 32) g4[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const float z[P::N] = {};
+        for (int k = lane; k < nv; k += 32) gv[k] = P::narrow(z);
         return;
     }
     const long long k0 = sk_index(c.b, c.t, c.u, maxU, SK);
@@ -202,20 +275,21 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const float* logits,
     const float gs = gscale ? gscale[c.b] : 1.f;
     const int label = (c.u < Un - 1) ? labels[(long long)c.b * (maxU - 1) + c.u] : -1;
     float sb = 0.f, sl = 0.f;
-    if (c.t == Tn - 1 && c.u == Un - 1) sb = expf(a + (x[blank] - l) - ll);
-    if (c.t < Tn - 1) sb = expf(a + (x[blank] - l) - ll + betas[k0 + maxU]);
-    if (label >= 0) sl = expf(a + (x[label] - l) - ll + betas[k0 + maxU + 1]);
+    if (c.t == Tn - 1 && c.u == Un - 1) sb = expf(a + (widen(x[blank]) - l) - ll);
+    if (c.t < Tn - 1) sb = expf(a + (widen(x[blank]) - l) - ll + betas[k0 + maxU]);
+    if (label >= 0) sl = expf(a + (widen(x[label]) - l) - ll + betas[k0 + maxU + 1]);
     const float kd = a + bt - ll - l;
-    for (int k = lane; k < n4; k += 32) {
-        const float4 v = x4[k];
-        float4 g = make_float4(expf(v.x + kd), expf(v.y + kd), expf(v.z + kd), expf(v.w + kd));
-        const int db = blank - (k << 2), dl = label - (k << 2);
-        g.x -= (db == 0 ? sb : 0.f) + (dl == 0 ? sl : 0.f);
-        g.y -= (db == 1 ? sb : 0.f) + (dl == 1 ? sl : 0.f);
-        g.z -= (db == 2 ? sb : 0.f) + (dl == 2 ? sl : 0.f);
-        g.w -= (db == 3 ? sb : 0.f) + (dl == 3 ? sl : 0.f);
-        g.x *= gs; g.y *= gs; g.z *= gs; g.w *= gs;
-        g4[k] = g;
+    for (int k = lane; k < nv; k += 32) {
+        float v[P::N], g[P::N];
+        P::widen(xv[k], v);
+#pragma unroll
+        for (int i = 0; i < P::N; ++i) g[i] = expf(v[i] + kd);
+        const int db = blank - (k << P::LOG2N), dl = label - (k << P::LOG2N);
+#pragma unroll
+        for (int i = 0; i < P::N; ++i) g[i] -= (db == i ? sb : 0.f) + (dl == i ? sl : 0.f);
+#pragma unroll
+        for (int i = 0; i < P::N; ++i) g[i] *= gs;
+        gv[k] = P::narrow(g);
     }
 }
 
@@ -338,10 +412,11 @@ __global__ void __launch_bounds__(1024) alpha_beta_kernel(const T* __restrict__ 
 //          - [v==blank & t<T-1] exp(alpha+lp_v-ll+beta(t+1,u)) - [v==label_u & u<U-1] exp(alpha+lp_v-ll+beta(t,u+1))
 // normalised by llForward (gpu_rnnt.h:198-200).  Padded cells are written 0 here (the reference
 // memsets the whole tensor first, gpu_rnnt.h:109).  `out` may alias `logits` (in-place, used by the
-// exact joint path).  gscale (nullable): per-utterance upstream gradient, pre-multiplied.
+// exact joint path).  gscale (nullable): per-utterance upstream gradient, pre-multiplied.  X: element type of the
+// logits and gradients (T, or fp16 / bf16 over a float workspace: one rounding, after the multiply).
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) rnnt_grad_kernel(const T* logits, T* out, long long row0, long long nrows,
+template <typename T, typename X = T>
+__global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out, long long row0, long long nrows,
                                                         int V, const int* __restrict__ xlen,
                                                         const int* __restrict__ ylen,
                                                         const int* __restrict__ labels, int maxT, int maxU,
@@ -354,10 +429,10 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const T* logits, T* out,
     const long long cell = row0 + row;
     const CellIdx c = decode_cell(cell, maxT, maxU);
     const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
-    const T* x = logits + row * (long long)V;
-    T* g = out + row * (long long)V;
+    const X* x = logits + row * (long long)V;
+    X* g = out + row * (long long)V;
     if (c.t >= Tn || c.u >= Un) {
-        for (int v = lane; v < V; v += 32) g[v] = T(0);
+        for (int v = lane; v < V; v += 32) g[v] = narrow<X>(T(0));
         return;
     }
     const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
@@ -365,15 +440,15 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const T* logits, T* out,
     const T gs = gscale ? gscale[c.b] : T(1);
     const int label = (c.u < Un - 1) ? labels[(long long)c.b * (maxU - 1) + c.u] : -1;
     T sb = 0, sl = 0;
-    if (c.t == Tn - 1 && c.u == Un - 1) sb = xexp(a + (x[blank] - l) - ll);
-    if (c.t < Tn - 1) sb = xexp(a + (x[blank] - l) - ll + betas[k + maxU]);        // beta(t+1,u): next diagonal, same column
-    if (label >= 0) sl = xexp(a + (x[label] - l) - ll + betas[k + maxU + 1]);      // beta(t,u+1): next diagonal, next column
+    if (c.t == Tn - 1 && c.u == Un - 1) sb = xexp(a + (widen(x[blank]) - l) - ll);
+    if (c.t < Tn - 1) sb = xexp(a + (widen(x[blank]) - l) - ll + betas[k + maxU]);        // beta(t+1,u): next diagonal, same column
+    if (label >= 0) sl = xexp(a + (widen(x[label]) - l) - ll + betas[k + maxU + 1]);      // beta(t,u+1): next diagonal, next column
     const T kd = a + bt - ll - l;
     for (int v = lane; v < V; v += 32) {
-        T gr = xexp(x[v] + kd);
+        T gr = xexp(widen(x[v]) + kd);
         if (v == blank) gr -= sb;
         if (v == label) gr -= sl;
-        g[v] = gr * gs;
+        g[v] = narrow<X>(gr * gs);
     }
 }
 

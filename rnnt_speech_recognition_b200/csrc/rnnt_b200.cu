@@ -73,10 +73,19 @@ rnntStatus_t launch_alpha_beta(const LossWs<T>& w, const int* xlen, const int* y
     return check_launch();
 }
 
-// loss op on materialised logits: lse+gather -> alpha/beta -> (grad).  costs stay on device in w.llf.
-template <typename T>
-rnntStatus_t loss_op(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, const T* gscale,
-                     int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+// The 16-byte fast paths need float workspace arithmetic, V a multiple of the elements per 16 bytes and 16-byte
+// aligned tensors (rows then stay aligned).
+template <typename T, typename X>
+bool vec_ok(const X* acts, const X* grads, int V) {
+    return sizeof(T) == 4 && (V % (16 / (int)sizeof(X))) == 0 && ((uintptr_t)acts % 16) == 0 &&
+           (!grads || ((uintptr_t)grads % 16) == 0);
+}
+
+// loss op on materialised logits, forward half: lse+gather -> alpha/beta.  costs stay on device in w.llf.
+// X is the logits' element type: T itself, or fp16 / bf16 over a float workspace.
+template <typename T, typename X>
+rnntStatus_t loss_planes(const X* acts, bool vec, const int* labels, const int* ylen, const int* xlen, int V, int B,
+                         int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
     if (maxU > 1024) {
         fprintf(stderr, "rnnt_b200: maxU=%d exceeds the 1024 label positions per utterance limit\n", maxU);
         return RNNT_STATUS_INVALID_VALUE;
@@ -84,38 +93,65 @@ rnntStatus_t loss_op(const T* acts, T* grads, const int* labels, const int* ylen
     LossWs<T> w(workspace, B, maxT, maxU);
     const long long N = (long long)B * maxT * maxU, SK = skew_plane(maxT, maxU);
     const unsigned blocks = (unsigned)((N * 32 + 255) / 256);
-    // 16-byte fast paths need float data, V % 4 == 0 and 16-byte aligned tensors (rows then stay aligned)
-    const bool vec = sizeof(T) == 4 && (V % 4) == 0 && ((uintptr_t)acts % 16) == 0 && (!grads || ((uintptr_t)grads % 16) == 0);
     {
         rb::ScopedTimer tm("lse_gather_kernel", s);
-        if (vec) {
-            if (V <= 1024)
-                rb::lse_gather_vec_kernel<8><<<blocks, 256, 0, s>>>((const float*)acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                                    blank, (float*)w.lse, (float*)w.lpb, (float*)w.lpl);
-            else
-                rb::lse_gather_vec_kernel<0><<<blocks, 256, 0, s>>>((const float*)acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                                    blank, (float*)w.lse, (float*)w.lpb, (float*)w.lpl);
-        } else {
-            rb::lse_gather_kernel<T><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
-                                                            w.lse, w.lpb, w.lpl);
+        if constexpr (sizeof(T) == 4) {
+            if (vec) {
+                if (V <= 8 * 32 * (16 / (int)sizeof(X)))      // 8 pieces of 16 bytes per lane held in registers
+                    rb::lse_gather_vec_kernel<X, 8><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
+                                                                           blank, w.lse, w.lpb, w.lpl);
+                else
+                    rb::lse_gather_vec_kernel<X, 0><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
+                                                                           blank, w.lse, w.lpb, w.lpl);
+            }
         }
+        if (!vec)
+            rb::lse_gather_kernel<T, X><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
+                                                               w.lse, w.lpb, w.lpl);
     }
     RB_LAUNCHED(1);
     if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
     if (launch_alpha_beta(w, xlen, ylen, B, maxT, maxU, s)) return RNNT_STATUS_EXECUTION_FAILED;
-    if (grads) {
-        rb::ScopedTimer tm("rnnt_grad_kernel", s);
-        if (vec)
-            rb::rnnt_grad_vec_kernel<<<blocks, 256, 0, s>>>((const float*)acts, (float*)grads, 0, N, V, xlen, ylen, labels, maxT,
-                                                            maxU, SK, blank, (const float*)w.lse, (const float*)w.alphas,
-                                                            (const float*)w.betas, (const float*)w.llf, (const float*)gscale);
-        else
-            rb::rnnt_grad_kernel<T><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                           blank, w.lse, w.alphas, w.betas, w.llf, gscale);
-        RB_LAUNCHED(1);
-        if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
-    }
     return RNNT_STATUS_SUCCESS;
+}
+
+// backward half: gradients w.r.t. the logits from the planes loss_planes left in the workspace
+template <typename T, typename X>
+rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, const int* ylen, const int* xlen,
+                        const T* gscale, int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+    LossWs<T> w(workspace, B, maxT, maxU);
+    const long long N = (long long)B * maxT * maxU, SK = skew_plane(maxT, maxU);
+    const unsigned blocks = (unsigned)((N * 32 + 255) / 256);
+    rb::ScopedTimer tm("rnnt_grad_kernel", s);
+    if constexpr (sizeof(T) == 4) {
+        if (vec)
+            rb::rnnt_grad_vec_kernel<X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
+                                                               w.lse, w.alphas, w.betas, w.llf, gscale);
+    }
+    if (!vec)
+        rb::rnnt_grad_kernel<T, X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
+                                                          blank, w.lse, w.alphas, w.betas, w.llf, gscale);
+    RB_LAUNCHED(1);
+    return check_launch();
+}
+
+// loss op on materialised logits: lse+gather -> alpha/beta -> (grad).  costs stay on device in w.llf.
+template <typename T>
+rnntStatus_t loss_op(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, const T* gscale,
+                     int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+    const bool vec = vec_ok<T>(acts, grads, V);
+    rnntStatus_t st = loss_planes<T, T>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s);
+    if (st || !grads) return st;
+    return loss_grads<T, T>(acts, grads, vec, labels, ylen, xlen, gscale, V, B, maxT, maxU, blank, workspace, s);
+}
+
+// argument checks of the 16-bit entries (those of rnntb200_loss_device, plus the logit type, the blank index and the
+// wavefront's maxU bound, so that the backward rejects what its forward would have)
+bool loss16_args_ok(const void* acts, int logit_type, const int* labels, const int* ylen, const int* xlen, int V, int B,
+                    const void* out, const void* workspace, const rnntOptions& o) {
+    return acts && labels && ylen && xlen && out && workspace && V > 0 && B > 0 && o.maxT > 0 && o.maxU > 0 &&
+           o.maxU <= 1024 && o.blank_label >= 0 && o.blank_label < V &&
+           (logit_type == RNNTB200_LOGITS_F16 || logit_type == RNNTB200_LOGITS_BF16);
 }
 
 template <typename T>
@@ -348,6 +384,53 @@ rnntStatus_t rnntb200_loss_device(const float* activations, float* gradients, co
     finish_costs_kernel<<<(minibatch + 127) / 128, 128, 0, s>>>(w.llf, w.llb, costs_device, minibatch);
     RB_LAUNCHED(1);
     return check_launch();
+}
+
+rnntStatus_t rnntb200_loss16_forward(const void* activations, int logit_type, const int* flat_labels,
+                                     const int* label_lengths, const int* input_lengths, int alphabet_size, int minibatch,
+                                     float* costs_device, void* workspace, rnntOptions options) {
+    if (!loss16_args_ok(activations, logit_type, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                        costs_device, workspace, options))
+        return RNNT_STATUS_INVALID_VALUE;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
+    const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
+    rnntStatus_t st;
+    if (logit_type == RNNTB200_LOGITS_F16) {
+        const __half* x = static_cast<const __half*>(activations);
+        st = loss_planes<float, __half>(x, vec_ok<float, __half>(x, nullptr, V), flat_labels, label_lengths, input_lengths,
+                                        V, B, T, U, blank, workspace, s);
+    } else {
+        const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(activations);
+        st = loss_planes<float, __nv_bfloat16>(x, vec_ok<float, __nv_bfloat16>(x, nullptr, V), flat_labels, label_lengths,
+                                               input_lengths, V, B, T, U, blank, workspace, s);
+    }
+    if (st) return st;
+    LossWs<float> w(workspace, B, T, U);
+    finish_costs_kernel<<<(B + 127) / 128, 128, 0, s>>>(w.llf, w.llb, costs_device, B);
+    RB_LAUNCHED(1);
+    return check_launch();
+}
+
+rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, const int* flat_labels,
+                                      const int* label_lengths, const int* input_lengths, const float* grad_costs,
+                                      int alphabet_size, int minibatch, void* gradients, const void* workspace,
+                                      rnntOptions options) {
+    if (!loss16_args_ok(activations, logit_type, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                        gradients, workspace, options))
+        return RNNT_STATUS_INVALID_VALUE;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
+    const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
+    void* ws = const_cast<void*>(workspace);      // read only: LossWs just carves the planes out of it
+    if (logit_type == RNNTB200_LOGITS_F16) {
+        const __half* x = static_cast<const __half*>(activations);
+        __half* g = static_cast<__half*>(gradients);
+        return loss_grads<float, __half>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, grad_costs,
+                                         V, B, T, U, blank, ws, s);
+    }
+    const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(activations);
+    __nv_bfloat16* g = static_cast<__nv_bfloat16*>(gradients);
+    return loss_grads<float, __nv_bfloat16>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths,
+                                            grad_costs, V, B, T, U, blank, ws, s);
 }
 
 rnntStatus_t rnntb200_joint_workspace_size(const rnntb200JointDesc* desc, size_t* size_bytes) {

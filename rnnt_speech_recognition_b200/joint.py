@@ -46,6 +46,13 @@ def _workspace(desc, device):
     return torch.empty(sz.value, dtype=torch.uint8, device=device)
 
 
+def _f32(t):
+    """Mixed-precision inputs (float16 / bfloat16, e.g. under torch.autocast) are cast to float32 at the boundary; the
+    kernels then run exactly as on float32 inputs, and autograd returns each gradient in its input's dtype.  Any other
+    dtype passes through (and is rejected by the checks)."""
+    return t.float() if t is not None and t.dtype in (torch.float16, torch.bfloat16) else t
+
+
 def _check(enc, pred, W, b, labels, input_lengths, label_lengths):
     for t, n in ((enc, "enc_acts"), (pred, "pred_acts"), (W, "W"), (b, "b")):
         if not t.is_cuda:
@@ -123,16 +130,18 @@ def joint_rnnt_loss(enc_acts, pred_acts, W, b, labels, input_lengths, label_leng
     (one more tensor-core pass).
     valid_tiles: optional promise `valid_tile_count(host lengths)` (rnntb200JointDesc.valid_tile_bound): sizes the workspace
     for the batch's valid lattice tiles instead of the padded (T,U) lattice, so that large ragged batches stay one chunk and
-    keep their numerators; a broken promise yields NaN costs and a device-side message, never an out-of-bounds write."""
-    return _JointRNNT.apply(enc_acts, pred_acts, W, b, labels, input_lengths, label_lengths, blank, precision, compact,
-                            keep_activations, valid_tiles)
+    keep their numerators; a broken promise yields NaN costs and a device-side message, never an out-of-bounds write.
+    float16 / bfloat16 inputs are cast to float32 first (costs float32, each gradient in its input's dtype)."""
+    return _JointRNNT.apply(_f32(enc_acts), _f32(pred_acts), _f32(W), _f32(b), labels, input_lengths, label_lengths, blank,
+                            precision, compact, keep_activations, valid_tiles)
 
 
 def joint_logits(enc_acts, pred_acts, W, b):
     """model.py:158-166's literal output: logits (B,T,U,V) float32, materialised (not differentiable;
-    use joint_rnnt_loss for training).  For callers that want the reference's tensor itself."""
+    use joint_rnnt_loss for training).  For callers that want the reference's tensor itself.  float16 / bfloat16
+    inputs are cast to float32; the logits are float32 either way."""
     L = _lib.load()
-    enc, pred, W, b = (t.contiguous() for t in (enc_acts, pred_acts, W, b))
+    enc, pred, W, b = (_f32(t).contiguous() for t in (enc_acts, pred_acts, W, b))
     B, T, H = enc.shape
     U, V = pred.shape[1], W.shape[1]
     with torch.cuda.device(enc.device):
@@ -148,8 +157,10 @@ def joint_step(f, g, K1, b1, K2, b2, want_logits=True, want_best=False):
     """``rnntb200_joint_step``: logits (B,V) of ONE lattice cell per batch row, tanh((f+g) @ K1 + b1) @ K2 + b2, and/or
     its argmax + log-softmax value.  ``f``, ``g``: (B,P) float32 CUDA views whose last dimension is contiguous (row
     strides are passed through, so ``encoded[:, i, :]`` / ``pred_out[:, -1, :]`` are not copied).  Not differentiable
-    (inference).  Returns (logits | None, best | None, best_logp | None)."""
+    (inference).  float16 / bfloat16 arguments are cast to float32 (outputs float32).
+    Returns (logits | None, best | None, best_logp | None)."""
     L = _lib.load()
+    f, g, K1, b1, K2, b2 = (_f32(t) for t in (f, g, K1, b1, K2, b2))
     for t, n in ((f, "f"), (g, "g"), (K2, "K2")):
         if not t.is_cuda or t.dtype != torch.float32:
             raise TypeError("%s must be a float32 CUDA tensor (rnnt_b200 has no CPU path)" % n)
@@ -215,8 +226,9 @@ class _Dense1(torch.autograd.Function):
 
 
 def dense1(x, K1, b1=None):
-    """``x @ K1 (+ b1)`` through the extension (differentiable in x, K1, b1)."""
-    return _Dense1.apply(x, K1, b1)
+    """``x @ K1 (+ b1)`` through the extension (differentiable in x, K1, b1).  float16 / bfloat16 arguments are cast to
+    float32 (output float32, each gradient in its argument's dtype)."""
+    return _Dense1.apply(_f32(x), _f32(K1), _f32(b1))
 
 
 class Joint(torch.nn.Module):

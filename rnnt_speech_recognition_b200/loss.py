@@ -21,7 +21,7 @@ def get_loss_fn(reduction_factor):
     _lib.load()  # fail loudly here, not with a fallback later
 
     def _loss_fn(y_true, y_pred, spec_lengths, label_lengths):
-        """y_true (B,U-1) int labels; y_pred (B,T,U,V) float32 logits; spec_lengths (B,) pre-reduction
+        """y_true (B,U-1) int labels; y_pred (B,T,U,V) float32 / float16 / bfloat16 logits; spec_lengths (B,) pre-reduction
         frame counts; label_lengths (B,) -> per-utterance NLL (B,).  utils/loss.py:24-36."""
         y_true = y_true.to(torch.int32).contiguous()                 # tf.cast(y_true, tf.int32)
         # GPU build: no explicit log_softmax (utils/loss.py:29-30 applies it only on CPU builds)

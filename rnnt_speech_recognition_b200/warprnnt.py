@@ -12,7 +12,9 @@ Differences from the reference bindings, all deliberate:
   * costs stay on the device (the reference copies them to host and synchronises the stream
     every call, gpu_rnnt.h:209-213; the torch binding builds a CPU tensor, __init__.py:27);
   * CUDA tensors only: the reference's CPU branch is not reproduced (no CPU fallback);
-  * gradients of padded cells are written by the gradient kernel itself (no memset pass).
+  * gradients of padded cells are written by the gradient kernel itself (no memset pass);
+  * float16 / bfloat16 logits are accepted natively (the reference's op is float32-only): fp32 arithmetic, costs
+    float32, gradients formed in the backward pass in the logits' dtype with the upstream gradient folded in.
 """
 import ctypes as C
 
@@ -120,20 +122,73 @@ class _RNNTOp(torch.autograd.Function):
         return g.mul_(grad_costs.view(-1, 1, 1, 1).to(g)), None, None, None, None
 
 
+_LOGIT_TYPE = {torch.float16: _lib.LOGITS_F16, torch.bfloat16: _lib.LOGITS_BF16}
+
+
+class _RNNTOp16(torch.autograd.Function):
+    """The op on float16 / bfloat16 logits (mixed-precision training).  The forward computes costs only and keeps the
+    fp32 workspace; the backward forms the 16-bit gradient in one pass with ``grad_costs`` multiplied in before its
+    single rounding, so a loss-scaled fp16 gradient does not underflow and no fp32 (B,T,U,V) tensor ever exists."""
+
+    @staticmethod
+    def forward(ctx, acts, labels, act_lens, label_lens, blank):
+        L = _lib.load()
+        for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
+            _require_cuda(t, n)
+        B, T, U, V = acts.shape
+        if labels.shape[1] != U - 1 and not (U == 1 and labels.shape[1] == 0):
+            raise ValueError("labels must be (B, U-1)")
+        costs = torch.empty(B, dtype=torch.float32, device=acts.device)
+        ws = torch.empty(workspace_bytes(T, U, B), dtype=torch.uint8, device=acts.device)
+        lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
+        with torch.cuda.device(acts.device):
+            opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, int(blank), T, U, True)
+            st = L.rnntb200_loss16_forward(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
+                                           _ptr(act_lens), V, B, _ptr(costs), _ptr(ws), opt)
+        _lib.check(st, "rnntb200_loss16_forward")
+        if acts.requires_grad:
+            ctx.save_for_backward(acts, lab, act_lens, label_lens)
+            ctx.ws, ctx.blank = ws, int(blank)
+        return costs
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_costs):
+        L = _lib.load()
+        acts, lab, act_lens, label_lens = ctx.saved_tensors
+        B, T, U, V = acts.shape
+        g = grad_costs.to(torch.float32).contiguous()
+        grads = torch.empty_like(acts)
+        with torch.cuda.device(acts.device):
+            opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, ctx.blank, T, U, True)
+            st = L.rnntb200_loss16_backward(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
+                                            _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws), opt)
+        _lib.check(st, "rnntb200_loss16_backward")
+        ctx.ws = None
+        return grads, None, None, None, None
+
+
+def _op(acts):
+    """float16 / bfloat16 logits take the native 16-bit op; everything else the float32 op (which rejects other types)."""
+    return _RNNTOp16 if acts.dtype in _LOGIT_TYPE else _RNNTOp
+
+
 def rnnt_loss(acts, labels, input_lengths, label_lengths, blank_label=0):
     """TF-binding signature (warprnnt_tensorflow/__init__.py:9): per-utterance costs (B,).
-    ``acts`` are raw logits (B,T,U,V) float32 -- the softmax is performed inside, as the reference's
-    GPU op does.  ``labels`` (B,U-1) int32 zero padded; lengths (B,) int32."""
+    ``acts`` are raw logits (B,T,U,V) float32, float16 or bfloat16 -- the softmax is performed inside, as the
+    reference's GPU op does; costs are float32 and ``acts.grad`` has ``acts.dtype``.  ``labels`` (B,U-1) int32 zero
+    padded; lengths (B,) int32."""
     acts = acts.contiguous()
     certify_inputs(acts, labels, input_lengths, label_lengths, check_max=False)
-    return _RNNTOp.apply(acts, labels, input_lengths, label_lengths, blank_label)
+    return _op(acts).apply(acts, labels, input_lengths, label_lengths, blank_label)
 
 
 def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean"):
     """warprnnt_pytorch.rnnt_loss (pytorch_binding/warprnnt_pytorch/__init__.py:53-70):
-    reduction in {'none','sum','mean'}; 'mean' divides the summed cost by the batch size."""
+    reduction in {'none','sum','mean'}; 'mean' divides the summed cost by the batch size.  ``acts`` float32, float16
+    or bfloat16 (costs float32 either way)."""
     certify_inputs(acts, labels, act_lens, label_lens, check_max=True)
-    costs = _RNNTOp.apply(acts, labels, act_lens, label_lens, blank)
+    costs = _op(acts).apply(acts, labels, act_lens, label_lens, blank)
     if reduction in ("sum", "mean"):
         costs = costs.sum().unsqueeze(-1)
         if reduction == "mean":
