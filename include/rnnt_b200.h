@@ -130,6 +130,20 @@ rnntStatus_t rnntb200_loss_device(const float* activations, float* gradients, co
                                   int alphabet_size, int minibatch, float* costs_device, void* workspace,
                                   rnntOptions options);
 
+/** FastEmit regularisation (Yu et al., "FastEmit: Low-latency Streaming ASR with Sequence-level Emission
+ *  Regularization", ICASSP 2021) on the entries that form gradients.  fastemit_lambda >= 0, finite, one value for the
+ *  batch: the gradient of every label-emission log-probability lp_label(t,u) is multiplied by (1 + lambda), blank
+ *  log-probabilities keep theirs.  w.r.t. the logits (softmax inside), with occupancy gamma, blank-arc term gamma_B and
+ *  label-arc occupancy gamma_L of a cell:
+ *    d cost / d logit[v] = (gamma + lambda*gamma_L) p_v - [v == blank] gamma_B - [v == label_u] (1 + lambda) gamma_L.
+ *  The COSTS ARE UNCHANGED (-log p(y|x), not (1 + lambda) times it), so loss curves compare across lambda.
+ *  fastemit_lambda == 0 gives results bit-identical to the entries without the suffix, which are these entries with 0.
+ *  A negative, NaN or infinite fastemit_lambda returns RNNT_STATUS_INVALID_VALUE before any device work. */
+rnntStatus_t rnntb200_loss_device_fastemit(const float* activations, float* gradients, const int* flat_labels,
+                                           const int* label_lengths, const int* input_lengths, const float* grad_scale,
+                                           int alphabet_size, int minibatch, float* costs_device, void* workspace,
+                                           rnntOptions options, float fastemit_lambda);
+
 /** Element type of 16-bit logits (mixed-precision training: fp16 / bf16 activations). */
 typedef enum {
     RNNTB200_LOGITS_F16 = 0,  /**< IEEE binary16 */
@@ -158,6 +172,12 @@ rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, c
                                       const int* label_lengths, const int* input_lengths, const float* grad_costs,
                                       int alphabet_size, int minibatch, void* gradients, const void* workspace,
                                       rnntOptions options);
+
+/** rnntb200_loss16_backward with FastEmit (see rnntb200_loss_device_fastemit); the forward call is unchanged. */
+rnntStatus_t rnntb200_loss16_backward_fastemit(const void* activations, int logit_type, const int* flat_labels,
+                                               const int* label_lengths, const int* input_lengths, const float* grad_costs,
+                                               int alphabet_size, int minibatch, void* gradients, const void* workspace,
+                                               rnntOptions options, float fastemit_lambda);
 
 typedef enum {
     RNNTB200_FP32_EXACT = 0, /**< fp32 CUDA-core arithmetic; parity gate rtol 1e-4 (BASELINE C1/C2) */
@@ -213,6 +233,14 @@ rnntStatus_t rnntb200_joint_loss_backward(const rnntb200JointDesc* desc, const f
                                           const int* label_lengths, const int* input_lengths,
                                           const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                           float* db, void* workspace);
+
+/** rnntb200_joint_loss_backward with FastEmit (see rnntb200_loss_device_fastemit), on both precisions; the forward call
+ *  is unchanged and the descriptor keeps its layout. */
+rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                   const float* W, const float* bias, const int* labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   const float* grad_costs, float* d_enc, float* d_pred, float* dW,
+                                                   float* db, void* workspace, float fastemit_lambda);
 
 /** Joint network forward only, materialising logits (B,maxT,maxU,V) fp32 -- the literal
  *  model.py:158-166 output, used by the drop-in `Joint` module when a caller wants the tensor

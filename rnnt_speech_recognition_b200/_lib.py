@@ -29,8 +29,10 @@ class JointDesc(C.Structure):
 
 EXPORTS = ("get_warprnnt_version", "rnntGetStatusString", "get_workspace_size", "compute_rnnt_loss",
            "compute_rnnt_loss_fp64", "rnntb200_loss_device", "rnntb200_loss16_forward", "rnntb200_loss16_backward",
+           "rnntb200_loss_device_fastemit", "rnntb200_loss16_backward_fastemit",
            "rnntb200_joint_workspace_size",
-           "rnntb200_joint_loss_forward", "rnntb200_joint_loss_backward", "rnntb200_joint_logits", "rnntb200_joint_step",
+           "rnntb200_joint_loss_forward", "rnntb200_joint_loss_backward", "rnntb200_joint_loss_backward_fastemit",
+           "rnntb200_joint_logits", "rnntb200_joint_step",
            "rnntb200_dense1_forward", "rnntb200_dense1_backward",
            "rnntb200_launch_count", "rnntb200_build_info", "rnntb200_set_timing", "rnntb200_get_timing")
 
@@ -66,9 +68,12 @@ def load(build_if_missing=True):
     L.rnntb200_loss_device.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
     L.rnntb200_loss16_forward.argtypes = [vp, ci, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
     L.rnntb200_loss16_backward.argtypes = [vp, ci, vp, vp, vp, vp, ci, ci, vp, vp, RnntOptions]
+    L.rnntb200_loss_device_fastemit.argtypes = L.rnntb200_loss_device.argtypes + [C.c_float]
+    L.rnntb200_loss16_backward_fastemit.argtypes = L.rnntb200_loss16_backward.argtypes + [C.c_float]
     L.rnntb200_joint_workspace_size.argtypes = [C.POINTER(JointDesc), C.POINTER(C.c_size_t)]
     L.rnntb200_joint_loss_forward.argtypes = [C.POINTER(JointDesc)] + [vp] * 9
     L.rnntb200_joint_loss_backward.argtypes = [C.POINTER(JointDesc)] + [vp] * 13
+    L.rnntb200_joint_loss_backward_fastemit.argtypes = L.rnntb200_joint_loss_backward.argtypes + [C.c_float]
     L.rnntb200_joint_logits.argtypes = [C.POINTER(JointDesc)] + [vp] * 6
     L.rnntb200_joint_step.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
     L.rnntb200_dense1_forward.argtypes = [vp, C.c_longlong, ci, vp, vp, ci, vp, vp]
@@ -80,6 +85,17 @@ def load(build_if_missing=True):
     L.rnntb200_get_timing.argtypes = [ci, C.POINTER(C.c_char_p), C.POINTER(C.c_float)]
     _lib = L
     return L
+
+
+def fastemit_lambda(value):
+    """FastEmit's lambda as the library takes it: a finite float >= 0 (ValueError otherwise)."""
+    try:
+        lam = float(value)
+    except (TypeError, ValueError):
+        raise ValueError("fastemit_lambda must be a finite number >= 0, got %r" % (value,)) from None
+    if not (0.0 <= lam < float("inf")):          # NaN fails the comparison too
+        raise ValueError("fastemit_lambda must be a finite number >= 0, got %r" % (value,))
+    return lam
 
 
 def check(status, what):

@@ -374,11 +374,12 @@ struct LossPlanes { const float *lse, *lpb, *lpl, *alphas, *betas, *llf; };   //
 // Backward (SURVEY 8 a19) with the library's own wgmma kernels (joint_bwd.cuh).  Per utterance chunk: (a keeping forward
 // of the chunk unless the forward call already kept the whole batch) -> row_scale_kernel -> bwd_dz_kernel -> d_pred plane
 // sum -> bwd_dw_kernel; after the last chunk the split-K planes of dW / db are summed.  Stream-ordered, no host
-// synchronisation, no library calls.
+// synchronisation, no library calls.  FastEmit lives entirely in row_scale_kernel (every chunk, keep or recompute): the
+// GEMM kernels consume E' as they always do.
 inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const float* enc, const float* pred,
                                 const float* bias, const int* labels, const int* ylen, const int* xlen,
                                 const LossPlanes& lp, const float* grad_costs, float* d_enc, float* d_pred, float* dW,
-                                float* db, cudaStream_t s, unsigned* launches) {
+                                float* db, cudaStream_t s, unsigned* launches, float fastemit_lambda) {
     if (!tc_supported(d)) return tc_unsupported(d);
     const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
     const DzGeom zg = dz_geometry(d.H);
@@ -409,7 +410,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
             row_scale_kernel<<<(unsigned)(((size_t)nb * g.nTb * g.nUb * 128 + 255) / 256), 256, 0, s>>>(
                 sc.tile_of_slot, sc.count, b0, g.nTb, g.nUb, xlen, ylen, labels, d.blank_label, d.maxT, d.maxU,
                 (long long)(d.maxT + d.maxU - 1) * d.maxU, lp.lse, lp.lpb, lp.lpl, lp.alphas, lp.betas, lp.llf, grad_costs, sc.gm,
-                d.V, reinterpret_cast<unsigned short*>(sc.dl), sc.rowscale);
+                d.V, reinterpret_cast<unsigned short*>(sc.dl), sc.rowscale, fastemit_lambda);
             *launches += 1;
         }
         BwdParams p{};

@@ -130,6 +130,16 @@ __device__ __forceinline__ T warp_sum(T v) {
     return v;
 }
 
+// FastEmit (Yu et al. 2021): the share of a cell's occupancy that leaves through its label arc,
+//   rho = exp(lp_label(t,u) + beta(t,u+1) - beta(t,u)) in [0, 1],
+// clamped to 1 so that rounding cannot push it above, and so that a cell with beta(t,u) = -inf (rho NaN or +inf; its
+// occupancy is 0) gets a finite factor 1 + lambda*rho.
+template <typename T>
+__device__ __forceinline__ T fastemit_rho(T lp_label, T beta_next_u, T beta) {
+    const T r = xexp(lp_label + beta_next_u - beta);
+    return r < T(1) ? r : T(1);
+}
+
 struct CellIdx { int b, t, u; };
 __device__ __forceinline__ CellIdx decode_cell(long long cell, int maxT, int maxU) {
     CellIdx c;
@@ -253,7 +263,7 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
                                                             const float* __restrict__ alphas,
                                                             const float* __restrict__ betas,
                                                             const float* __restrict__ llf,
-                                                            const float* __restrict__ gscale) {
+                                                            const float* __restrict__ gscale, float fastemit_lambda) {
     using P = Vec16<X>;
     const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -278,7 +288,12 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
     if (c.t == Tn - 1 && c.u == Un - 1) sb = expf(a + (widen(x[blank]) - l) - ll);
     if (c.t < Tn - 1) sb = expf(a + (widen(x[blank]) - l) - ll + betas[k0 + maxU]);
     if (label >= 0) sl = expf(a + (widen(x[label]) - l) - ll + betas[k0 + maxU + 1]);
-    const float kd = a + bt - ll - l;
+    float kd = a + bt - ll - l;
+    if (fastemit_lambda != 0.f && label >= 0) {       // FastEmit: see rnnt_grad_kernel
+        const float rho = fastemit_rho(widen(x[label]) - l, betas[k0 + maxU + 1], bt);
+        kd += log1pf(fastemit_lambda * rho);
+        sl *= 1.f + fastemit_lambda;
+    }
     for (int k = lane; k < nv; k += 32) {
         float v[P::N], g[P::N];
         P::widen(xv[k], v);
@@ -414,6 +429,10 @@ __global__ void __launch_bounds__(1024) alpha_beta_kernel(const T* __restrict__ 
 // memsets the whole tensor first, gpu_rnnt.h:109).  `out` may alias `logits` (in-place, used by the
 // exact joint path).  gscale (nullable): per-utterance upstream gradient, pre-multiplied.  X: element type of the
 // logits and gradients (T, or fp16 / bf16 over a float workspace: one rounding, after the multiply).
+// FastEmit (fastemit_lambda > 0): the label arc's gradient is scaled by (1 + lambda), so the row becomes
+//   g[v] = (gamma + lambda*gamma_L) p_v - [v==blank] gamma_B - [v==label_u] (1 + lambda) gamma_L,
+// gamma_L = sl; the softmax term is today's times (1 + lambda*rho) (fastemit_rho), i.e. kd += log1p(lambda*rho).
+// lambda == 0 takes none of this arithmetic: the result is bit-identical to the plain loss.
 // ---------------------------------------------------------------------------------------------
 template <typename T, typename X = T>
 __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out, long long row0, long long nrows,
@@ -422,7 +441,8 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
                                                         const int* __restrict__ labels, int maxT, int maxU,
                                                         long long SK, int blank, const T* __restrict__ lse,
                                                         const T* __restrict__ alphas, const T* __restrict__ betas,
-                                                        const T* __restrict__ llf, const T* __restrict__ gscale) {
+                                                        const T* __restrict__ llf, const T* __restrict__ gscale,
+                                                        float fastemit_lambda) {
     const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
@@ -443,7 +463,12 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
     if (c.t == Tn - 1 && c.u == Un - 1) sb = xexp(a + (widen(x[blank]) - l) - ll);
     if (c.t < Tn - 1) sb = xexp(a + (widen(x[blank]) - l) - ll + betas[k + maxU]);        // beta(t+1,u): next diagonal, same column
     if (label >= 0) sl = xexp(a + (widen(x[label]) - l) - ll + betas[k + maxU + 1]);      // beta(t,u+1): next diagonal, next column
-    const T kd = a + bt - ll - l;
+    T kd = a + bt - ll - l;
+    if (fastemit_lambda != 0.f && label >= 0) {
+        const T lam = fastemit_lambda;
+        kd += xlog1p(lam * fastemit_rho<T>(widen(x[label]) - l, betas[k + maxU + 1], bt));
+        sl *= T(1) + lam;
+    }
     for (int v = lane; v < V; v += 32) {
         T gr = xexp(widen(x[v]) + kd);
         if (v == blank) gr -= sb;
@@ -459,6 +484,8 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
 // except for v = blank and v = label_u, whose outgoing-arc terms (gpu_rnnt_kernel.h:163-172) are subtracted: their FINAL
 // values dl_blank, dl_label are formed here from the cached log-probs and stored as E' = dl / rs in place of E, so that
 // rs * E' is exact for them too.  Rows outside the valid lattice get rs = 0 (their E stays finite: it was formed from z = 0).
+// FastEmit (fastemit_lambda > 0, see rnnt_grad_kernel): rs is multiplied by fe = 1 + lambda*rho and the label arc's term
+// by 1 + lambda, which the patched columns absorb; lambda == 0 leaves fe = 1 and every value bit-identical.
 __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ tile_of_slot, const int* __restrict__ count, int b0,
                                                         int nTb, int nUb, const int* __restrict__ xlen, const int* __restrict__ ylen,
                                                         const int* __restrict__ labels, int blank, int maxT, int maxU, long long SK,
@@ -466,7 +493,8 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
                                                         const float* __restrict__ lpl, const float* __restrict__ alphas,
                                                         const float* __restrict__ betas, const float* __restrict__ llf,
                                                         const float* __restrict__ gscale, const float* __restrict__ rowref, int V,
-                                                        unsigned short* __restrict__ E, float* __restrict__ rowscale) {
+                                                        unsigned short* __restrict__ E, float* __restrict__ rowscale,
+                                                        float fastemit_lambda) {
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int sl = (int)(row >> 7), r = (int)(row & 127);
     if (sl >= *count) return;
@@ -485,9 +513,14 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
         const bool has_label = u < Un - 1;
         int lab = -1;
         if (has_label) { sl_ = expf(a + lpl[k] - ll + betas[k + maxU + 1]); pl = expf(lpl[k] + occ); lab = labels[(long long)b * (maxU - 1) + u]; }
-        float dlb = g * (expf(lpb[k] + occ) - sb), dll = g * (pl - sl_);
+        float fe = 1.f;                                                  // FastEmit factor of the softmax term
+        if (fastemit_lambda != 0.f && has_label) {
+            fe = 1.f + fastemit_lambda * fastemit_rho(lpl[k], betas[k + maxU + 1], bt);
+            sl_ *= 1.f + fastemit_lambda;
+        }
+        float dlb = g * (fe * expf(lpb[k] + occ) - sb), dll = g * (fe * pl - sl_);
         if (has_label && lab == blank) { dlb -= g * sl_; dll = dlb; }    // degenerate: label == blank
-        rs = g * exp2f(rowref[row] + (occ - lse[((long long)b * maxT + t) * maxU + u]) * 1.4426950408889634f);
+        rs = fe * (g * exp2f(rowref[row] + (occ - lse[((long long)b * maxT + t) * maxU + u]) * 1.4426950408889634f));
         // rs is cut to 0 only where 1/rs stops being finite (a denormal rs would make it +inf and the patched columns NaN).
         // The forward keeps lse2 - ref <= FWD_REBASE + log2 V, so a row cut here has |g| * e^occ < 2^-126 * 2^(64 + log2 V):
         // at V = 4096 below 2^-50, against rows of up to |g|.  The patched columns dl / rs are at most 2^(lse2 - ref),

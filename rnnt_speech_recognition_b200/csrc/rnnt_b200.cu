@@ -7,6 +7,7 @@
 #include <climits>
 #include <cstdio>
 #include <cstdint>
+#include <cfloat>
 #include <cmath>
 #include <vector>
 
@@ -118,7 +119,8 @@ rnntStatus_t loss_planes(const X* acts, bool vec, const int* labels, const int* 
 // backward half: gradients w.r.t. the logits from the planes loss_planes left in the workspace
 template <typename T, typename X>
 rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, const int* ylen, const int* xlen,
-                        const T* gscale, int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+                        const T* gscale, int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s,
+                        float fastemit_lambda) {
     LossWs<T> w(workspace, B, maxT, maxU);
     const long long N = (long long)B * maxT * maxU, SK = skew_plane(maxT, maxU);
     const unsigned blocks = (unsigned)((N * 32 + 255) / 256);
@@ -126,11 +128,11 @@ rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, co
     if constexpr (sizeof(T) == 4) {
         if (vec)
             rb::rnnt_grad_vec_kernel<X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
-                                                               w.lse, w.alphas, w.betas, w.llf, gscale);
+                                                               w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda);
     }
     if (!vec)
         rb::rnnt_grad_kernel<T, X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                          blank, w.lse, w.alphas, w.betas, w.llf, gscale);
+                                                          blank, w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda);
     RB_LAUNCHED(1);
     return check_launch();
 }
@@ -138,11 +140,12 @@ rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, co
 // loss op on materialised logits: lse+gather -> alpha/beta -> (grad).  costs stay on device in w.llf.
 template <typename T>
 rnntStatus_t loss_op(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, const T* gscale,
-                     int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+                     int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s, float fastemit_lambda) {
     const bool vec = vec_ok<T>(acts, grads, V);
     rnntStatus_t st = loss_planes<T, T>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s);
     if (st || !grads) return st;
-    return loss_grads<T, T>(acts, grads, vec, labels, ylen, xlen, gscale, V, B, maxT, maxU, blank, workspace, s);
+    return loss_grads<T, T>(acts, grads, vec, labels, ylen, xlen, gscale, V, B, maxT, maxU, blank, workspace, s,
+                            fastemit_lambda);
 }
 
 // argument checks of the 16-bit entries (those of rnntb200_loss_device, plus the logit type, the blank index and the
@@ -153,6 +156,9 @@ bool loss16_args_ok(const void* acts, int logit_type, const int* labels, const i
            o.maxU <= 1024 && o.blank_label >= 0 && o.blank_label < V &&
            (logit_type == RNNTB200_LOGITS_F16 || logit_type == RNNTB200_LOGITS_BF16);
 }
+
+// FastEmit's lambda: finite and >= 0 (NaN fails both comparisons)
+inline bool fastemit_ok(float lambda) { return lambda >= 0.f && lambda <= FLT_MAX; }
 
 template <typename T>
 rnntStatus_t compute_impl(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, int V, int B,
@@ -168,7 +174,7 @@ rnntStatus_t compute_impl(const T* acts, T* grads, const int* labels, const int*
     if (opt.loc != RNNT_GPU) return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(opt.stream);
     rnntStatus_t st = loss_op<T>(acts, grads, labels, ylen, xlen, nullptr, V, B, opt.maxT, opt.maxU, opt.blank_label,
-                                 workspace, s);
+                                 workspace, s, 0.f);
     if (st) return st;
     // costs to HOST + sync + negate, as gpu_rnnt.h:209-213; llBackward comes along for the guard of cpu_rnnt.h:166-170
     LossWs<T> w(workspace, B, opt.maxT, opt.maxU);
@@ -284,7 +290,7 @@ rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const 
 rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
                             const float* W, const float* bias, const int* labels, const int* ylen, const int* xlen,
                             const float* grad_costs, float* d_enc, float* d_pred, float* dW, float* db,
-                            cudaStream_t s) {
+                            cudaStream_t s, float fastemit_lambda) {
     const long long N = (long long)d.B * d.maxT * d.maxU, SK = skew_plane(d.maxT, d.maxU);
     float* Z = reinterpret_cast<float*>(ws.scratch);
     float* L = Z + ws.chunk_rows * d.H;
@@ -301,7 +307,7 @@ rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const
         // dlogits in place (gpu_rnnt_kernel.h:143-179 formula, times the upstream per-utterance gradient)
         rb::rnnt_grad_kernel<float><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
             L, L, r0, rows, d.V, xlen, ylen, labels, d.maxT, d.maxU, SK, d.blank_label, ws.loss.lse, ws.loss.alphas,
-            ws.loss.betas, ws.loss.llf, grad_costs);
+            ws.loss.betas, ws.loss.llf, grad_costs, fastemit_lambda);
         // dZ = dL . W^T      (rows x V) . (V x H):  B(k=v, n=h) = W[h*V + v]
         {
             rb::ScopedTimer tm("sgemm dZ=dL.W^T", s);
@@ -372,13 +378,21 @@ rnntStatus_t rnntb200_loss_device(const float* activations, float* gradients, co
                                   const int* label_lengths, const int* input_lengths, const float* grad_scale,
                                   int alphabet_size, int minibatch, float* costs_device, void* workspace,
                                   rnntOptions options) {
+    return rnntb200_loss_device_fastemit(activations, gradients, flat_labels, label_lengths, input_lengths, grad_scale,
+                                         alphabet_size, minibatch, costs_device, workspace, options, 0.f);
+}
+
+rnntStatus_t rnntb200_loss_device_fastemit(const float* activations, float* gradients, const int* flat_labels,
+                                           const int* label_lengths, const int* input_lengths, const float* grad_scale,
+                                           int alphabet_size, int minibatch, float* costs_device, void* workspace,
+                                           rnntOptions options, float fastemit_lambda) {
     if (!activations || !flat_labels || !label_lengths || !input_lengths || !costs_device || !workspace ||
-        alphabet_size <= 0 || minibatch <= 0 || options.maxT <= 0 || options.maxU <= 0)
+        alphabet_size <= 0 || minibatch <= 0 || options.maxT <= 0 || options.maxU <= 0 || !fastemit_ok(fastemit_lambda))
         return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     rnntStatus_t st = loss_op<float>(activations, gradients, flat_labels, label_lengths, input_lengths, grad_scale,
                                      alphabet_size, minibatch, options.maxT, options.maxU, options.blank_label,
-                                     workspace, s);
+                                     workspace, s, fastemit_lambda);
     if (st) return st;
     LossWs<float> w(workspace, minibatch, options.maxT, options.maxU);
     finish_costs_kernel<<<(minibatch + 127) / 128, 128, 0, s>>>(w.llf, w.llb, costs_device, minibatch);
@@ -415,8 +429,16 @@ rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, c
                                       const int* label_lengths, const int* input_lengths, const float* grad_costs,
                                       int alphabet_size, int minibatch, void* gradients, const void* workspace,
                                       rnntOptions options) {
+    return rnntb200_loss16_backward_fastemit(activations, logit_type, flat_labels, label_lengths, input_lengths, grad_costs,
+                                             alphabet_size, minibatch, gradients, workspace, options, 0.f);
+}
+
+rnntStatus_t rnntb200_loss16_backward_fastemit(const void* activations, int logit_type, const int* flat_labels,
+                                               const int* label_lengths, const int* input_lengths, const float* grad_costs,
+                                               int alphabet_size, int minibatch, void* gradients, const void* workspace,
+                                               rnntOptions options, float fastemit_lambda) {
     if (!loss16_args_ok(activations, logit_type, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                        gradients, workspace, options))
+                        gradients, workspace, options) || !fastemit_ok(fastemit_lambda))
         return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
@@ -425,12 +447,12 @@ rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, c
         const __half* x = static_cast<const __half*>(activations);
         __half* g = static_cast<__half*>(gradients);
         return loss_grads<float, __half>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, grad_costs,
-                                         V, B, T, U, blank, ws, s);
+                                         V, B, T, U, blank, ws, s, fastemit_lambda);
     }
     const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(activations);
     __nv_bfloat16* g = static_cast<__nv_bfloat16*>(gradients);
     return loss_grads<float, __nv_bfloat16>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths,
-                                            grad_costs, V, B, T, U, blank, ws, s);
+                                            grad_costs, V, B, T, U, blank, ws, s, fastemit_lambda);
 }
 
 rnntStatus_t rnntb200_joint_workspace_size(const rnntb200JointDesc* desc, size_t* size_bytes) {
@@ -484,20 +506,29 @@ rnntStatus_t rnntb200_joint_loss_backward(const rnntb200JointDesc* desc, const f
                                           const int* label_lengths, const int* input_lengths,
                                           const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                           float* db, void* workspace) {
+    return rnntb200_joint_loss_backward_fastemit(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, grad_costs,
+                                                 d_enc, d_pred, dW, db, workspace, 0.f);
+}
+
+rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                   const float* W, const float* bias, const int* labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   const float* grad_costs, float* d_enc, float* d_pred, float* dW,
+                                                   float* db, void* workspace, float fastemit_lambda) {
     if (!desc_ok(desc) || !enc || !pred || !W || !bias || !labels || !label_lengths || !input_lengths ||
-        !grad_costs || !d_enc || !d_pred || !dW || !db || !workspace)
+        !grad_costs || !d_enc || !d_pred || !dW || !db || !workspace || !fastemit_ok(fastemit_lambda))
         return RNNT_STATUS_INVALID_VALUE;
     const rnntb200JointDesc& d = *desc;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
     JointWs ws(d, workspace);
     if (d.precision == RNNTB200_FP32_EXACT)
         return exact_backward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, grad_costs, d_enc,
-                              d_pred, dW, db, s);
+                              d_pred, dW, db, s, fastemit_lambda);
 #ifndef RNNTB200_NO_TC
     unsigned nl = 0;
     const rb::LossPlanes lp{ws.loss.lse, ws.loss.lpb, ws.loss.lpl, ws.loss.alphas, ws.loss.betas, ws.loss.llf};
     rnntStatus_t st = rb::tc_backward(d, ws.scratch, enc, pred, bias, labels, label_lengths, input_lengths, lp, grad_costs,
-                                      d_enc, d_pred, dW, db, s, &nl);
+                                      d_enc, d_pred, dW, db, s, &nl, fastemit_lambda);
     RB_LAUNCHED(nl);
     return st;
 #else

@@ -78,7 +78,8 @@ def _check(enc, pred, W, b, labels, input_lengths, label_lengths):
 
 class _JointRNNT(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, compact, keep=None, valid_tiles=None):
+    def forward(ctx, enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, compact, keep=None, valid_tiles=None,
+                fastemit_lambda=0.0):
         L = _lib.load()
         enc, pred, W, b = (t.contiguous() for t in (enc, pred, W, b))
         labels, input_lengths, label_lengths = (t.contiguous() for t in (labels, input_lengths, label_lengths))
@@ -97,7 +98,7 @@ class _JointRNNT(torch.autograd.Function):
         _lib.check(st, "rnntb200_joint_loss_forward")
         ctx.save_for_backward(enc, pred, W, b, lab, input_lengths, label_lengths)
         ctx.ws, ctx.dims, ctx.blank, ctx.precision, ctx.compact, ctx.keep = ws, (B, T, U, H, V), blank, precision, compact, keep
-        ctx.valid_tiles = valid_tiles
+        ctx.valid_tiles, ctx.fastemit_lambda = valid_tiles, fastemit_lambda
         return costs
 
     @staticmethod
@@ -109,16 +110,16 @@ class _JointRNNT(torch.autograd.Function):
         d_enc, d_pred, dW, db = (torch.empty_like(t) for t in (enc, pred, W, b))
         with torch.cuda.device(enc.device):
             desc = _desc(B, T, U, H, V, ctx.blank, ctx.precision, ctx.keep, ctx.valid_tiles)
-            st = L.rnntb200_joint_loss_backward(C.byref(desc), _ptr(enc), _ptr(pred), _ptr(W), _ptr(b), _ptr(lab),
-                                                _ptr(label_lengths), _ptr(input_lengths), _ptr(g), _ptr(d_enc),
-                                                _ptr(d_pred), _ptr(dW), _ptr(db), _ptr(ctx.ws))
-        _lib.check(st, "rnntb200_joint_loss_backward")
+            st = L.rnntb200_joint_loss_backward_fastemit(C.byref(desc), _ptr(enc), _ptr(pred), _ptr(W), _ptr(b), _ptr(lab),
+                                                         _ptr(label_lengths), _ptr(input_lengths), _ptr(g), _ptr(d_enc),
+                                                         _ptr(d_pred), _ptr(dW), _ptr(db), _ptr(ctx.ws), ctx.fastemit_lambda)
+        _lib.check(st, "rnntb200_joint_loss_backward_fastemit")
         ctx.ws = None
-        return d_enc, d_pred, dW, db, None, None, None, None, None, None, None, None
+        return d_enc, d_pred, dW, db, None, None, None, None, None, None, None, None, None
 
 
 def joint_rnnt_loss(enc_acts, pred_acts, W, b, labels, input_lengths, label_lengths, blank=0, precision="bf16",
-                    compact=True, keep_activations=None, valid_tiles=None):
+                    compact=True, keep_activations=None, valid_tiles=None, fastemit_lambda=0.0):
     """Per-utterance RNN-T NLL (B,) of logits = tanh(enc_acts[:,:,None]+pred_acts[:,None]) @ W + b,
     differentiable w.r.t. enc_acts, pred_acts, W, b -- without ever materialising (B,T,U,V).
     precision: 'bf16' = the tensor-core path (wgmma, 16-bit operands, fp32 accumulate) or 'fp32' (exact CUDA-core path).
@@ -131,9 +132,13 @@ def joint_rnnt_loss(enc_acts, pred_acts, W, b, labels, input_lengths, label_leng
     valid_tiles: optional promise `valid_tile_count(host lengths)` (rnntb200JointDesc.valid_tile_bound): sizes the workspace
     for the batch's valid lattice tiles instead of the padded (T,U) lattice, so that large ragged batches stay one chunk and
     keep their numerators; a broken promise yields NaN costs and a device-side message, never an out-of-bounds write.
-    float16 / bfloat16 inputs are cast to float32 first (costs float32, each gradient in its input's dtype)."""
+    float16 / bfloat16 inputs are cast to float32 first (costs float32, each gradient in its input's dtype).
+    fastemit_lambda: FastEmit regularisation (Yu et al. 2021), a finite float >= 0 (ValueError otherwise): the gradient
+    of every label-emission log-probability is scaled by (1 + lambda); the costs stay -log p(y|x).  0 = the plain loss,
+    bit for bit."""
+    lam = _lib.fastemit_lambda(fastemit_lambda)
     return _JointRNNT.apply(_f32(enc_acts), _f32(pred_acts), _f32(W), _f32(b), labels, input_lengths, label_lengths, blank,
-                            precision, compact, keep_activations, valid_tiles)
+                            precision, compact, keep_activations, valid_tiles, lam)
 
 
 def joint_logits(enc_acts, pred_acts, W, b):
@@ -236,9 +241,10 @@ class Joint(torch.nn.Module):
     dense_1 kernel (P,H) + bias (H) with tanh, dense_2 kernel (H,V) + bias (V).
 
     ``forward(inp_enc, pred_outputs)`` returns the reference's logits tensor (drop-in for the Keras
-    model output); ``loss(...)`` runs the fused path where that tensor never exists."""
+    model output); ``loss(...)`` runs the fused path where that tensor never exists, with FastEmit regularisation of
+    strength ``fastemit_lambda`` (0: none; see ``joint_rnnt_loss``)."""
 
-    def __init__(self, proj_size, joint_net_size, vocab_size, precision="bf16", blank=0):
+    def __init__(self, proj_size, joint_net_size, vocab_size, precision="bf16", blank=0, fastemit_lambda=0.0):
         super().__init__()
         self.kernel_1 = torch.nn.Parameter(torch.empty(proj_size, joint_net_size))
         self.bias_1 = torch.nn.Parameter(torch.zeros(joint_net_size))
@@ -247,6 +253,7 @@ class Joint(torch.nn.Module):
         torch.nn.init.xavier_uniform_(self.kernel_1)   # Keras Dense default glorot_uniform
         torch.nn.init.xavier_uniform_(self.kernel_2)
         self.precision, self.blank = precision, blank
+        self.fastemit_lambda = _lib.fastemit_lambda(fastemit_lambda)
 
     def hoist(self, inp_enc, pred_outputs):
         """Dense-1 is linear before its tanh, so it is applied to the (B,T,P) and (B,U,P) inputs instead of the (B,T,U,P)
@@ -274,7 +281,7 @@ class Joint(torch.nn.Module):
     def loss(self, inp_enc, pred_outputs, labels, input_lengths, label_lengths):
         enc_acts, pred_acts = self.hoist(inp_enc, pred_outputs)
         return joint_rnnt_loss(enc_acts, pred_acts, self.kernel_2, self.bias_2, labels, input_lengths, label_lengths,
-                               self.blank, self.precision)
+                               self.blank, self.precision, fastemit_lambda=self.fastemit_lambda)
 
 
 def get_fused_loss_fn(reduction_factor, joint):

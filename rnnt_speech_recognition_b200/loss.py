@@ -17,7 +17,9 @@ def encoder_lengths(spec_lengths, reduction_factor):
     return torch.ceil(spec_lengths.to(torch.float64) / reduction_factor).to(torch.int32)
 
 
-def get_loss_fn(reduction_factor):
+def get_loss_fn(reduction_factor, fastemit_lambda=0.0):
+    """``fastemit_lambda`` >= 0: FastEmit regularisation of the gradient (``rnnt_loss``); the costs are unchanged."""
+    lam = _lib.fastemit_lambda(fastemit_lambda)
     _lib.load()  # fail loudly here, not with a fallback later
 
     def _loss_fn(y_true, y_pred, spec_lengths, label_lengths):
@@ -26,6 +28,6 @@ def get_loss_fn(reduction_factor):
         y_true = y_true.to(torch.int32).contiguous()                 # tf.cast(y_true, tf.int32)
         # GPU build: no explicit log_softmax (utils/loss.py:29-30 applies it only on CPU builds)
         enc_lengths = encoder_lengths(spec_lengths, reduction_factor).contiguous()
-        return rnnt_loss(y_pred, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous())
+        return rnnt_loss(y_pred, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous(), fastemit_lambda=lam)
 
     return _loss_fn

@@ -14,7 +14,10 @@ Differences from the reference bindings, all deliberate:
   * CUDA tensors only: the reference's CPU branch is not reproduced (no CPU fallback);
   * gradients of padded cells are written by the gradient kernel itself (no memset pass);
   * float16 / bfloat16 logits are accepted natively (the reference's op is float32-only): fp32 arithmetic, costs
-    float32, gradients formed in the backward pass in the logits' dtype with the upstream gradient folded in.
+    float32, gradients formed in the backward pass in the logits' dtype with the upstream gradient folded in;
+  * ``fastemit_lambda`` (FastEmit, Yu et al. 2021; default 0 = the plain loss): the gradient of every label-emission
+    log-probability is scaled by (1 + lambda).  Costs stay -log p(y|x), not (1 + lambda) times it, so loss curves
+    compare across lambda.
 """
 import ctypes as C
 
@@ -93,7 +96,7 @@ class _RNNTOp(torch.autograd.Function):
     as both reference bindings do (warprnnt_op.cc:100-137, warprnnt_pytorch/__init__.py:24-42)."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
         L = _lib.load()
         for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
             _require_cuda(t, n)
@@ -109,9 +112,9 @@ class _RNNTOp(torch.autograd.Function):
         lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
         with torch.cuda.device(acts.device):     # the stream must be the current stream OF THE TENSORS' DEVICE
             opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, int(blank), T, U, True)
-            st = L.rnntb200_loss_device(_ptr(acts), _ptr(grads), _ptr(lab), _ptr(label_lens), _ptr(act_lens), None,
-                                        V, B, _ptr(costs), _ptr(ws), opt)
-        _lib.check(st, "rnntb200_loss_device")
+            st = L.rnntb200_loss_device_fastemit(_ptr(acts), _ptr(grads), _ptr(lab), _ptr(label_lens), _ptr(act_lens),
+                                                 None, V, B, _ptr(costs), _ptr(ws), opt, fastemit_lambda)
+        _lib.check(st, "rnntb200_loss_device_fastemit")
         ctx.grads = grads
         return costs
 
@@ -119,7 +122,7 @@ class _RNNTOp(torch.autograd.Function):
     def backward(ctx, grad_costs):
         g = ctx.grads
         ctx.grads = None
-        return g.mul_(grad_costs.view(-1, 1, 1, 1).to(g)), None, None, None, None
+        return g.mul_(grad_costs.view(-1, 1, 1, 1).to(g)), None, None, None, None, None
 
 
 _LOGIT_TYPE = {torch.float16: _lib.LOGITS_F16, torch.bfloat16: _lib.LOGITS_BF16}
@@ -131,7 +134,7 @@ class _RNNTOp16(torch.autograd.Function):
     single rounding, so a loss-scaled fp16 gradient does not underflow and no fp32 (B,T,U,V) tensor ever exists."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
         L = _lib.load()
         for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
             _require_cuda(t, n)
@@ -148,7 +151,7 @@ class _RNNTOp16(torch.autograd.Function):
         _lib.check(st, "rnntb200_loss16_forward")
         if acts.requires_grad:
             ctx.save_for_backward(acts, lab, act_lens, label_lens)
-            ctx.ws, ctx.blank = ws, int(blank)
+            ctx.ws, ctx.blank, ctx.fastemit_lambda = ws, int(blank), fastemit_lambda
         return costs
 
     @staticmethod
@@ -161,11 +164,12 @@ class _RNNTOp16(torch.autograd.Function):
         grads = torch.empty_like(acts)
         with torch.cuda.device(acts.device):
             opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, ctx.blank, T, U, True)
-            st = L.rnntb200_loss16_backward(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
-                                            _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws), opt)
-        _lib.check(st, "rnntb200_loss16_backward")
+            st = L.rnntb200_loss16_backward_fastemit(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
+                                                     _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws), opt,
+                                                     ctx.fastemit_lambda)
+        _lib.check(st, "rnntb200_loss16_backward_fastemit")
         ctx.ws = None
-        return grads, None, None, None, None
+        return grads, None, None, None, None, None
 
 
 def _op(acts):
@@ -173,22 +177,25 @@ def _op(acts):
     return _RNNTOp16 if acts.dtype in _LOGIT_TYPE else _RNNTOp
 
 
-def rnnt_loss(acts, labels, input_lengths, label_lengths, blank_label=0):
+def rnnt_loss(acts, labels, input_lengths, label_lengths, blank_label=0, fastemit_lambda=0.0):
     """TF-binding signature (warprnnt_tensorflow/__init__.py:9): per-utterance costs (B,).
     ``acts`` are raw logits (B,T,U,V) float32, float16 or bfloat16 -- the softmax is performed inside, as the
     reference's GPU op does; costs are float32 and ``acts.grad`` has ``acts.dtype``.  ``labels`` (B,U-1) int32 zero
-    padded; lengths (B,) int32."""
+    padded; lengths (B,) int32.  ``fastemit_lambda`` >= 0 (finite; ValueError otherwise): FastEmit regularisation of
+    the gradient, costs unchanged."""
+    lam = _lib.fastemit_lambda(fastemit_lambda)
     acts = acts.contiguous()
     certify_inputs(acts, labels, input_lengths, label_lengths, check_max=False)
-    return _op(acts).apply(acts, labels, input_lengths, label_lengths, blank_label)
+    return _op(acts).apply(acts, labels, input_lengths, label_lengths, blank_label, lam)
 
 
-def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean"):
+def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean", fastemit_lambda=0.0):
     """warprnnt_pytorch.rnnt_loss (pytorch_binding/warprnnt_pytorch/__init__.py:53-70):
     reduction in {'none','sum','mean'}; 'mean' divides the summed cost by the batch size.  ``acts`` float32, float16
-    or bfloat16 (costs float32 either way)."""
+    or bfloat16 (costs float32 either way).  ``fastemit_lambda``: as in ``rnnt_loss``."""
+    lam = _lib.fastemit_lambda(fastemit_lambda)
     certify_inputs(acts, labels, act_lens, label_lens, check_max=True)
-    costs = _op(acts).apply(acts, labels, act_lens, label_lens, blank)
+    costs = _op(acts).apply(acts, labels, act_lens, label_lens, blank, lam)
     if reduction in ("sum", "mean"):
         costs = costs.sum().unsqueeze(-1)
         if reduction == "mean":
@@ -201,10 +208,11 @@ def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean
 class RNNTLoss(torch.nn.Module):
     """warprnnt_pytorch.RNNTLoss (pytorch_binding/warprnnt_pytorch/__init__.py:73-100)."""
 
-    def __init__(self, blank=0, reduction="mean"):
+    def __init__(self, blank=0, reduction="mean", fastemit_lambda=0.0):
         super().__init__()
         self.blank = blank
         self.reduction = reduction
+        self.fastemit_lambda = _lib.fastemit_lambda(fastemit_lambda)
 
     def forward(self, acts, labels, act_lens, label_lens):
-        return torch_rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction)
+        return torch_rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda)
