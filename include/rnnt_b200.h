@@ -242,6 +242,41 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
                                                    const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                                    float* db, void* workspace, float fastemit_lambda);
 
+/** Forced alignment: the single most likely path through the lattice the loss sums over (Viterbi), per utterance b
+ *  with T = input_lengths[b], U = label_lengths[b] + 1 and the log-probs of the loss, lpb(t,u) at blank and lpl(t,u)
+ *  at labels[b][u]:
+ *    delta(0,0) = 0
+ *    delta(t,u) = max(delta(t-1,u) + lpb(t-1,u), delta(t,u-1) + lpl(t,u-1))   (a predecessor outside the lattice: -inf)
+ *    best_logp[b] = delta(T-1,U-1) + lpb(T-1,U-1)  <=  -costs[b]
+ *  Ties: the label arc wins only when it is STRICTLY greater, so on an exact tie the blank predecessor wins -- among
+ *  equally scoring paths the one that emits every label earliest.
+ *  label_frames (B, maxU-1) int32 device, row stride maxU-1: label_frames[b][j] is the frame t at which the best path
+ *  takes the label arc (t,j) -> (t,j+1), i.e. emits labels[b][j]; -1 for j >= U-1.  Per utterance the frames are
+ *  non-decreasing and lie in [0, T).  label_frames may be NULL only when maxU == 1.
+ *  costs / best_logp (B) float device.  The costs are those of the matching forward entry, bit for bit.
+ *  Not differentiable; the workspace (same size as the forward's) is overwritten with the decisions and cannot feed a
+ *  backward call.  Stream-ordered, no allocation, no host synchronisation (CUDA-graph capturable).  Errors as the
+ *  matching forward entry, plus maxU > 1024 and a blank outside [0, V) -> RNNT_STATUS_INVALID_VALUE before any device
+ *  work.
+ *  rnntb200_align_device: fp32 logits, arguments of rnntb200_loss_device (workspace of get_workspace_size). */
+rnntStatus_t rnntb200_align_device(const float* activations, const int* flat_labels, const int* label_lengths,
+                                   const int* input_lengths, int alphabet_size, int minibatch, float* costs_device,
+                                   float* best_logp, int* label_frames, void* workspace, rnntOptions options);
+
+/** Forced alignment on 16-bit logits (arguments of rnntb200_loss16_forward; fp32 arithmetic). */
+rnntStatus_t rnntb200_align16(const void* activations, int logit_type, const int* flat_labels, const int* label_lengths,
+                              const int* input_lengths, int alphabet_size, int minibatch, float* costs_device,
+                              float* best_logp, int* label_frames, void* workspace, rnntOptions options);
+
+/** Forced alignment on the fused joint path (arguments of rnntb200_joint_loss_forward, workspace of
+ *  rnntb200_joint_workspace_size), both precisions; the (B,T,U,V) logits are never written.  keep_activations is
+ *  ignored (nothing is kept).  valid_tile_bound is honoured: a broken promise gives NaN costs, NaN best_logp and
+ *  label_frames of -1. */
+rnntStatus_t rnntb200_joint_align(const rnntb200JointDesc* desc, const float* enc, const float* pred, const float* W,
+                                  const float* bias, const int* labels, const int* label_lengths,
+                                  const int* input_lengths, float* costs, float* best_logp, int* label_frames,
+                                  void* workspace);
+
 /** Joint network forward only, materialising logits (B,maxT,maxU,V) fp32 -- the literal
  *  model.py:158-166 output, used by the drop-in `Joint` module when a caller wants the tensor
  *  (e.g. to feed rnnt_loss/compute_rnnt_loss exactly as run_rnnt.py:269-273 does). */

@@ -32,6 +32,7 @@ EXPORTS = ("get_warprnnt_version", "rnntGetStatusString", "get_workspace_size", 
            "rnntb200_loss_device_fastemit", "rnntb200_loss16_backward_fastemit",
            "rnntb200_joint_workspace_size",
            "rnntb200_joint_loss_forward", "rnntb200_joint_loss_backward", "rnntb200_joint_loss_backward_fastemit",
+           "rnntb200_align_device", "rnntb200_align16", "rnntb200_joint_align",
            "rnntb200_joint_logits", "rnntb200_joint_step",
            "rnntb200_dense1_forward", "rnntb200_dense1_backward",
            "rnntb200_launch_count", "rnntb200_build_info", "rnntb200_set_timing", "rnntb200_get_timing")
@@ -74,6 +75,9 @@ def load(build_if_missing=True):
     L.rnntb200_joint_loss_forward.argtypes = [C.POINTER(JointDesc)] + [vp] * 9
     L.rnntb200_joint_loss_backward.argtypes = [C.POINTER(JointDesc)] + [vp] * 13
     L.rnntb200_joint_loss_backward_fastemit.argtypes = L.rnntb200_joint_loss_backward.argtypes + [C.c_float]
+    L.rnntb200_align_device.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, RnntOptions]
+    L.rnntb200_align16.argtypes = [vp, ci, vp, vp, vp, ci, ci, vp, vp, vp, vp, RnntOptions]
+    L.rnntb200_joint_align.argtypes = [C.POINTER(JointDesc)] + [vp] * 11
     L.rnntb200_joint_logits.argtypes = [C.POINTER(JointDesc)] + [vp] * 6
     L.rnntb200_joint_step.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
     L.rnntb200_dense1_forward.argtypes = [vp, C.c_longlong, ci, vp, vp, ci, vp, vp]

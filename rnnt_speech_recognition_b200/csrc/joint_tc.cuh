@@ -369,6 +369,21 @@ inline rnntStatus_t tc_forward(const rnntb200JointDesc& d, void* scratch, const 
     return tc_run_forward<false>(d, g, sc, enc, pred, bias, labels, ylen, xlen, lse, lpb, lpl, 0, d.B, s, launches);
 }
 
+// The valid_tile_bound promise of a call that keeps nothing (alignment): when a bound is given and the batch is one
+// workspace chunk, the tiles are counted as the keeping forward counts them.  Returns the overflow word (nonzero:
+// the promise is broken) or nullptr when there is nothing to check.
+inline const int* tc_check_tile_bound(const rnntb200JointDesc& d, void* scratch, const int* ylen, const int* xlen,
+                                      cudaStream_t s, unsigned* launches) {
+    if (d.valid_tile_bound <= 0 || !tc_supported(d)) return nullptr;
+    const TcScratch sc = tc_scratch_layout(d, scratch);
+    if (sc.bchunk < d.B) return nullptr;
+    const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
+    tile_compact_kernel<<<1, 1024, 0, s>>>(xlen, ylen, 0, d.B * g.nTb * g.nUb, g.nTb, g.nUb, g.TT, g.UU, sc.slot, sc.count,
+                                           nullptr, nullptr, d.maxT, d.maxU, (int)(sc.rows_chunk / 128));
+    *launches += 1;
+    return sc.count + 1;
+}
+
 struct LossPlanes { const float *lse, *lpb, *lpl, *alphas, *betas, *llf; };   // outputs of the forward + alpha/beta (loss workspace)
 
 // Backward (SURVEY 8 a19) with the library's own wgmma kernels (joint_bwd.cuh).  Per utterance chunk: (a keeping forward

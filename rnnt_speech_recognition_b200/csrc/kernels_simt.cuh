@@ -319,11 +319,18 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
 //   alpha(t,u) = LSE(alpha(t-1,u)+lpb(t-1,u), alpha(t,u-1)+lpl(t,u-1))        cpu_rnnt.h:182-195
 //   beta(t,u)  = LSE(beta(t+1,u)+lpb(t,u),    beta(t,u+1)+lpl(t,u))            cpu_rnnt.h:223-236
 //   llForward  = alpha(T-1,U-1)+lpb(T-1,U-1); llBackward = beta(0,0)           cpu_rnnt.h:209,251
+// VIT (forward direction only) runs the same walk in the max-plus semiring: the Viterbi recurrence of forced alignment,
+//   delta(t,u) = max(delta(t-1,u)+lpb(t-1,u), delta(t,u-1)+lpl(t,u-1)),   ll = delta(T-1,U-1)+lpb(T-1,U-1),
+// with delta kept in registers only (`out` is not written).  Each warp records its decisions of a diagonal as ONE 32-bit
+// ballot word, bit (u & 31) set when the label arc is STRICTLY greater (a tie goes to the blank arc):
+//   dec[b*SKW + n*decw + (u >> 5)],  SKW = (maxT+maxU-1)*decw,  decw = ceil(maxU / 32).
 // ---------------------------------------------------------------------------------------------
-template <typename T, int PF, bool BETA>
+template <typename T, int PF, bool BETA, bool VIT = false>
 __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const T* __restrict__ lpl, T* __restrict__ out,
                                                 T* __restrict__ ll, const int* __restrict__ xlen,
-                                                const int* __restrict__ ylen, int maxU, long long SK) {
+                                                const int* __restrict__ ylen, int maxU, long long SK,
+                                                unsigned* __restrict__ dec = nullptr, int decw = 0) {
+    static_assert(!(VIT && BETA), "the Viterbi walk runs forward");
     const int b = blockIdx.x;
     const int u = threadIdx.x, lane = u & 31, warp = u >> 5;
     const int Tn = xlen[b], Un = ylen[b] + 1;
@@ -358,6 +365,8 @@ __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const
     const int nmacro = (nsteps + PF - 1) / PF + (multi ? nwarps - 1 : 0);
     // step i works on diagonal n = i (alpha) / nsteps - 1 - i (beta): row n of the skewed planes, one pointer bump per step
     const long long dstep = BETA ? -(long long)maxU : (long long)maxU;
+    // VIT: this warp's decision word of diagonal 0, one row of decw words per diagonal
+    unsigned* pdec = VIT ? dec + (long long)b * (long long)(SK / maxU) * decw + warp : nullptr;
     T cb[PF], cl[PF], nb[PF], nl[PF];
     auto fetch = [&](int i0, T* vb, T* vl) {
 #pragma unroll
@@ -387,7 +396,14 @@ __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const
                 const bool active = col_ok && t >= 0 && t < Tn;
                 const T vb = cb[j], vl = cl[j];
                 T val;
-                if (!BETA) {
+                if (VIT) {
+                    // delta(t,u) and its decision: the label arc wins only when strictly greater
+                    const T emit = (u > 0) ? nbr : NEG;
+                    const bool lab = emit > own;
+                    val = (i == 0) ? T(0) : (lab ? emit : own);
+                    const unsigned word = __ballot_sync(0xffffffffu, lab);
+                    if (lane == 0 && warp < nwarps) pdec[(long long)i * decw] = word;
+                } else if (!BETA) {
                     // alpha(t,u); own == -inf when t == 0, nbr is unused (forced -inf) when u == 0
                     const T emit = (u > 0) ? nbr : NEG;
                     val = (i == 0) ? T(0) : wave_lse(emit, own);
@@ -397,7 +413,7 @@ __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const
                     val = (t == Tn - 1 && u == Un - 1) ? vb : wave_lse(emit, no_emit);
                 }
                 if (active) {
-                    *po = val;
+                    if (!VIT) *po = val;
                     own = BETA ? val : val + vb;
                     pass = BETA ? val : val + vl;
                     result = own;      // alpha, last cell: alpha(T-1,U-1)+lpb(T-1,U-1);  beta, cell (0,0): beta(0,0)
@@ -419,6 +435,67 @@ __global__ void __launch_bounds__(1024) alpha_beta_kernel(const T* __restrict__ 
                                                           const int* __restrict__ ylen, int maxU, long long SK) {
     if (blockIdx.y == 1) alpha_beta_body<T, PF, true>(lpb, lpl, betas, llb, xlen, ylen, maxU, SK);
     else alpha_beta_body<T, PF, false>(lpb, lpl, alphas, llf, xlen, ylen, maxU, SK);
+}
+
+// Forced alignment, step 1: the Viterbi wavefront (alpha_beta_body<VIT>), one CTA per utterance.  Writes the decision
+// bit-plane `dec` and best[b] = delta(T-1,U-1)+lpb(T-1,U-1), the log-probability of the single best alignment.
+template <int PF>
+__global__ void __launch_bounds__(1024) viterbi_kernel(const float* __restrict__ lpb, const float* __restrict__ lpl,
+                                                       unsigned* __restrict__ dec, float* __restrict__ best,
+                                                       const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                                       int maxU, long long SK) {
+    alpha_beta_body<float, PF, false, true>(lpb, lpl, nullptr, best, xlen, ylen, maxU, SK, dec, (maxU + 31) >> 5);
+}
+
+// Forced alignment, step 2: the backtrace, one CTA per utterance.  The walk from (T-1,U-1) to (0,0) moves down exactly
+// one diagonal per step, so the decision rows it reads are known before it starts: they are streamed into shared memory
+// in chunks of BT_WORDS words, warps 1.. loading chunk c+1 while lane 0 of warp 0 walks chunk c, and every step of the
+// walk costs one shared-memory read instead of a dependent L2 round trip.  On the lattice's edges the only predecessor
+// is taken (t == 0: the label arc, u == 0: the blank arc), whatever the bit says.
+//   frames[b*(maxU-1) + j] = t of the label arc (t,j) -> (t,j+1) on the best path;  -1 for j >= U_b - 1.
+// overflow (nullable): the tensor-core forward's broken valid_tile_bound word: best = NaN and every frame -1.
+constexpr int BT_THREADS = 256, BT_WORDS = 4096;
+__global__ void __launch_bounds__(BT_THREADS) backtrace_kernel(const unsigned* __restrict__ dec, const float* __restrict__ vbest,
+                                                               const int* __restrict__ overflow, const int* __restrict__ xlen,
+                                                               const int* __restrict__ ylen, int maxT, int maxU,
+                                                               float* __restrict__ best_logp, int* __restrict__ frames) {
+    __shared__ unsigned buf[2][BT_WORDS];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const int Tn = xlen[b], Un = ylen[b] + 1;
+    const int decw = (maxU + 31) >> 5, wn = (Un + 31) >> 5;      // words per diagonal: stored / used by this utterance
+    const bool bad = overflow && *overflow;
+    int* fr = frames + (long long)b * (maxU - 1);
+    for (int j = (bad ? 0 : Un - 1) + tid; j < maxU - 1; j += BT_THREADS) fr[j] = -1;
+    if (tid == 0) best_logp[b] = bad ? __int_as_float(0x7fc00000) : vbest[b];
+    if (bad) return;
+    const unsigned* db = dec + (long long)b * (maxT + maxU - 1) * decw;
+    const int top = Tn + Un - 2;                 // the walk reads diagonals top, top-1, ..., 1
+    const int rows = BT_WORDS / wn;              // diagonals per chunk
+    const int nchunks = (top + rows - 1) / rows;
+    // chunk c holds diagonals top - c*rows down to max(1, top - (c+1)*rows + 1), word k at row top - c*rows - k / wn
+    auto load = [&](int c, unsigned* dst, int l0, int nl) {
+        const int hi = top - c * rows, lo = max(1, hi - rows + 1), n = (hi - lo + 1) * wn;
+        for (int k = tid - l0; k < n; k += nl) {
+            const int r = k / wn;
+            dst[k] = db[(long long)(hi - r) * decw + (k - r * wn)];
+        }
+    };
+    if (nchunks > 0) load(0, buf[0], 0, BT_THREADS);
+    __syncthreads();
+    int t = Tn - 1, u = Un - 1;
+    for (int c = 0; c < nchunks; ++c) {
+        if (tid >= 32 && c + 1 < nchunks) load(c + 1, buf[(c + 1) & 1], 32, BT_THREADS - 32);
+        if (tid == 0) {
+            const unsigned* s = buf[c & 1];
+            const int hi = top - c * rows, lo = max(1, hi - rows + 1);
+            for (int n = hi; n >= lo; --n) {
+                const unsigned w = s[(hi - n) * wn + (u >> 5)];
+                if (u > 0 && (t == 0 || ((w >> (u & 31)) & 1u))) { --u; fr[u] = t; }
+                else --t;
+            }
+        }
+        __syncthreads();
+    }
 }
 
 // ---------------------------------------------------------------------------------------------

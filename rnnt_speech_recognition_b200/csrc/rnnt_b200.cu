@@ -74,6 +74,31 @@ rnntStatus_t launch_alpha_beta(const LossWs<T>& w, const int* xlen, const int* y
     return check_launch();
 }
 
+// Forced alignment over the lp_blank / lp_label planes of a finished forward: the Viterbi wavefront, then the backtrace.
+// The costs are final by now (finish_costs_kernel ran), so the decision bit-plane, (maxT+maxU-1) * ceil(maxU/32) words
+// per utterance, goes into the beta plane ((maxT+maxU-1) * maxU floats) and delta's end value into llb: the workspace
+// keeps its size, and cannot feed a backward call afterwards.
+rnntStatus_t launch_align(const LossWs<float>& w, const int* xlen, const int* ylen, int B, int maxT, int maxU,
+                          const int* overflow, float* best_logp, int* frames, cudaStream_t s) {
+    unsigned* dec = reinterpret_cast<unsigned*>(w.betas);
+    {
+        rb::ScopedTimer tm("viterbi_kernel", s);
+        rb::viterbi_kernel<8><<<B, (maxU + 31) / 32 * 32, 0, s>>>(w.lpb, w.lpl, dec, w.llb, xlen, ylen, maxU,
+                                                                  skew_plane(maxT, maxU));
+    }
+    RB_LAUNCHED(1);
+    if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
+    {
+        rb::ScopedTimer tm("backtrace_kernel", s);
+        rb::backtrace_kernel<<<B, rb::BT_THREADS, 0, s>>>(dec, w.llb, overflow, xlen, ylen, maxT, maxU, best_logp, frames);
+    }
+    RB_LAUNCHED(1);
+    return check_launch();
+}
+
+// argument checks the three align entries add to those of their forward entries
+inline bool align_args_ok(const float* best_logp, const int* frames, int maxU) { return best_logp && (frames || maxU == 1); }
+
 // The 16-byte fast paths need float workspace arithmetic, V a multiple of the elements per 16 bytes and 16-byte
 // aligned tensors (rows then stay aligned).
 template <typename T, typename X>
@@ -535,6 +560,68 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
     fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
     return RNNT_STATUS_EXECUTION_FAILED;
 #endif
+}
+
+rnntStatus_t rnntb200_align_device(const float* activations, const int* flat_labels, const int* label_lengths,
+                                   const int* input_lengths, int alphabet_size, int minibatch, float* costs_device,
+                                   float* best_logp, int* label_frames, void* workspace, rnntOptions options) {
+    if (!align_args_ok(best_logp, label_frames, options.maxU) || options.maxU > 1024 || options.blank_label < 0 ||
+        options.blank_label >= alphabet_size)
+        return RNNT_STATUS_INVALID_VALUE;
+    rnntStatus_t st = rnntb200_loss_device(activations, nullptr, flat_labels, label_lengths, input_lengths, nullptr,
+                                           alphabet_size, minibatch, costs_device, workspace, options);
+    if (st) return st;
+    LossWs<float> w(workspace, minibatch, options.maxT, options.maxU);
+    return launch_align(w, input_lengths, label_lengths, minibatch, options.maxT, options.maxU, nullptr, best_logp,
+                        label_frames, reinterpret_cast<cudaStream_t>(options.stream));
+}
+
+rnntStatus_t rnntb200_align16(const void* activations, int logit_type, const int* flat_labels, const int* label_lengths,
+                              const int* input_lengths, int alphabet_size, int minibatch, float* costs_device,
+                              float* best_logp, int* label_frames, void* workspace, rnntOptions options) {
+    if (!align_args_ok(best_logp, label_frames, options.maxU)) return RNNT_STATUS_INVALID_VALUE;
+    rnntStatus_t st = rnntb200_loss16_forward(activations, logit_type, flat_labels, label_lengths, input_lengths,
+                                              alphabet_size, minibatch, costs_device, workspace, options);
+    if (st) return st;
+    LossWs<float> w(workspace, minibatch, options.maxT, options.maxU);
+    return launch_align(w, input_lengths, label_lengths, minibatch, options.maxT, options.maxU, nullptr, best_logp,
+                        label_frames, reinterpret_cast<cudaStream_t>(options.stream));
+}
+
+rnntStatus_t rnntb200_joint_align(const rnntb200JointDesc* desc, const float* enc, const float* pred, const float* W,
+                                  const float* bias, const int* labels, const int* label_lengths,
+                                  const int* input_lengths, float* costs, float* best_logp, int* label_frames,
+                                  void* workspace) {
+    if (!desc_ok(desc) || !enc || !pred || !W || !bias || !labels || !label_lengths || !input_lengths || !costs ||
+        !workspace || !align_args_ok(best_logp, label_frames, desc->maxU))
+        return RNNT_STATUS_INVALID_VALUE;
+    rnntb200JointDesc d = *desc;
+    d.keep_activations = 0;                 // no backward follows: nothing beyond the loss planes is kept
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
+    JointWs ws(d, workspace);
+    const int* overflow = nullptr;
+    rnntStatus_t st;
+    if (d.precision == RNNTB200_FP32_EXACT) {
+        st = exact_forward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, s);
+    } else {
+#ifndef RNNTB200_NO_TC
+        unsigned nl = 0;
+        st = rb::tc_forward(d, ws.scratch, enc, pred, W, bias, labels, label_lengths, input_lengths, ws.loss.lse,
+                            ws.loss.lpb, ws.loss.lpl, s, &nl);
+        if (!st) overflow = rb::tc_check_tile_bound(d, ws.scratch, label_lengths, input_lengths, s, &nl);
+        RB_LAUNCHED(nl);
+#else
+        fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
+        st = RNNT_STATUS_EXECUTION_FAILED;
+#endif
+    }
+    if (st) return st;
+    st = launch_alpha_beta(ws.loss, input_lengths, label_lengths, d.B, d.maxT, d.maxU, s);
+    if (st) return st;
+    finish_costs_kernel<<<(d.B + 127) / 128, 128, 0, s>>>(ws.loss.llf, ws.loss.llb, costs, d.B, overflow);
+    RB_LAUNCHED(1);
+    if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
+    return launch_align(ws.loss, input_lengths, label_lengths, d.B, d.maxT, d.maxU, overflow, best_logp, label_frames, s);
 }
 
 rnntStatus_t rnntb200_joint_logits(const rnntb200JointDesc* desc, const float* enc, const float* pred,

@@ -283,6 +283,16 @@ class Joint(torch.nn.Module):
         return joint_rnnt_loss(enc_acts, pred_acts, self.kernel_2, self.bias_2, labels, input_lengths, label_lengths,
                                self.blank, self.precision, fastemit_lambda=self.fastemit_lambda)
 
+    @torch.no_grad()
+    def align(self, inp_enc, pred_outputs, labels, input_lengths, label_lengths):
+        """Forced alignment on the fused path (``joint_rnnt_align``): the frame at which the most likely path emits each
+        label.  Returns ``Alignment(label_frames, best_logp, costs)``; the costs equal ``loss``'s.  FastEmit does not
+        change it: lambda touches only gradients."""
+        from .align import joint_rnnt_align
+        enc_acts, pred_acts = self.hoist(inp_enc, pred_outputs)
+        return joint_rnnt_align(enc_acts, pred_acts, self.kernel_2, self.bias_2, labels, input_lengths, label_lengths,
+                                self.blank, self.precision)
+
 
 def get_fused_loss_fn(reduction_factor, joint):
     """utils/loss.get_loss_fn-shaped adapter for the fused path: the returned function takes the joint
