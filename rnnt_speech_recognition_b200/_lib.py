@@ -102,6 +102,17 @@ def fastemit_lambda(value):
     return lam
 
 
+def ptr(t):
+    """A tensor's device address as the C ABI takes it (None: NULL)."""
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def stream():
+    """The current CUDA stream (of the current device: call inside ``with torch.cuda.device(...)``)."""
+    import torch
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
 def check(status, what):
     if status != 0:
         raise RuntimeError("%s failed: %s (status %d)" % (what, load().rnntGetStatusString(status).decode(), status))

@@ -22,8 +22,9 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .joint import _check, _desc, _f32, _workspace
-from .warprnnt import _LOGIT_TYPE, _ptr, _require_cuda, _stream, certify_inputs, workspace_bytes
+from ._lib import ptr as _ptr
+from .joint import _f32, _joint_setup
+from .warprnnt import _LOGIT_TYPE, _options, _prepare, certify_inputs
 
 __all__ = ["Alignment", "rnnt_align", "joint_rnnt_align"]
 
@@ -46,16 +47,10 @@ def rnnt_align(acts, labels, act_lens, label_lens, blank=0):
     L = _lib.load()
     acts = acts.contiguous()
     certify_inputs(acts, labels, act_lens, label_lens, check_max=False)
-    for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
-        _require_cuda(t, n)
-    B, T, U, V = acts.shape
-    if labels.shape[1] != U - 1 and not (U == 1 and labels.shape[1] == 0):
-        raise ValueError("labels must be (B, U-1)")
+    (B, T, U, V), ws, lab = _prepare(acts, labels, act_lens, label_lens)
     frames, best, costs = _outputs(B, U, acts.device)
-    ws = torch.empty(workspace_bytes(T, U, B), dtype=torch.uint8, device=acts.device)
-    lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
     with torch.cuda.device(acts.device):
-        opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, int(blank), T, U, True)
+        opt = _options(blank, T, U)
         if acts.dtype == torch.float32:
             name = "rnntb200_align_device"
             st = L.rnntb200_align_device(_ptr(acts), _ptr(lab), _ptr(label_lens), _ptr(act_lens), V, B, _ptr(costs),
@@ -76,18 +71,11 @@ def joint_rnnt_align(enc_acts, pred_acts, W, b, labels, input_lengths, label_len
     ``valid_tiles`` promise gives NaN costs and best_logp and frames of -1).  Returns ``Alignment``; its costs equal
     those of ``joint_rnnt_loss`` with the same precision, bit for bit."""
     L = _lib.load()
-    enc, pred, W, b = (_f32(t).contiguous() for t in (enc_acts, pred_acts, W, b))
-    labels, input_lengths, label_lengths = (t.contiguous() for t in (labels, input_lengths, label_lengths))
-    _check(enc, pred, W, b, labels, input_lengths, label_lengths)
-    B, T, H = enc.shape
-    U, V = pred.shape[1], W.shape[1]
-    lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=enc.device)
-    with torch.cuda.device(enc.device):
-        desc = _desc(B, T, U, H, V, blank, precision, False, valid_tiles)
-        ws = _workspace(desc, enc.device)
-        frames, best, costs = _outputs(B, U, enc.device)
-        st = L.rnntb200_joint_align(C.byref(desc), _ptr(enc), _ptr(pred), _ptr(W), _ptr(b), _ptr(lab),
-                                    _ptr(label_lengths), _ptr(input_lengths), _ptr(costs), _ptr(best), _ptr(frames),
-                                    _ptr(ws))
+    args, desc, ws = _joint_setup(_f32(enc_acts), _f32(pred_acts), _f32(W), _f32(b), labels, input_lengths, label_lengths,
+                                  blank, precision, False, valid_tiles)
+    device = args[0].device
+    frames, best, costs = _outputs(desc.B, desc.maxU, device)
+    with torch.cuda.device(device):
+        st = L.rnntb200_joint_align(C.byref(desc), *map(_ptr, args), _ptr(costs), _ptr(best), _ptr(frames), _ptr(ws))
     _lib.check(st, "rnntb200_joint_align")
     return Alignment(frames, best, costs)

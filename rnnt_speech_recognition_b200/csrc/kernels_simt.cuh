@@ -9,8 +9,9 @@
 //   rnnt_grad_kernel    gradient w.r.t. logits (gpu_rnnt_kernel.h:143-179), padded cells zeroed
 //                       in the same pass (replaces the cudaMemsetAsync of gpu_rnnt.h:109)
 //   row_scale_kernel    per-row scales of the tensor-core backward GEMMs + the patch of the two special columns
-//   zgen/sgemm/...      fp32 building blocks of the exact (RNNTB200_FP32_EXACT) joint path
-// lse_gather and rnnt_grad also take fp16 / bf16 logits (and write gradients of that type) over fp32 arithmetic.
+//   zgen/sgemm/...      fp32 building blocks of the exact (RNNTB200_FP32_EXACT) joint path, and colsum (also dense1's db1)
+// lse_gather and rnnt_grad also take fp16 / bf16 logits (and write gradients of that type) over fp32 arithmetic; their
+// scalar and 16-byte (_vec) kernels share row_cell (and store_lse_logprobs); arc_terms serves rnnt_grad[_vec] and row_scale.
 //
 // Data layout ("skewed" planes): a per-utterance plane stores cell (t,u) at row n=t+u, column u:
 //     sk(b,t,u) = b*SK + (t+u)*maxU + u,   SK = (maxT+maxU-1)*maxU
@@ -153,6 +154,56 @@ __device__ __forceinline__ long long sk_index(int b, int t, int u, int maxU, lon
     return (long long)b * SK + (long long)(t + u) * maxU + u;
 }
 
+// Prologue of the one-warp-per-row kernels (lse_gather, rnnt_grad): the warp's row of the chunk, and its lattice cell
+// (natural cell row0 + row) with the utterance's extent.  A padded cell (t >= T_b or u >= U_b) is never read downstream.
+__device__ __forceinline__ long long warp_row() { return ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
+struct RowCell {
+    long long cell;
+    int b, t, u, Tn, Un;
+    __device__ bool padded() const { return t >= Tn || u >= Un; }
+    __device__ long long sk(int maxU, long long SK) const { return sk_index(b, t, u, maxU, SK); }
+    // labels[b][u], -1 on the last column (no label arc)
+    __device__ int label(const int* labels, int maxU) const { return u < Un - 1 ? labels[(long long)b * (maxU - 1) + u] : -1; }
+};
+__device__ __forceinline__ RowCell row_cell(long long cell, int maxT, int maxU, const int* xlen, const int* ylen) {
+    const CellIdx c = decode_cell(cell, maxT, maxU);
+    return {cell, c.b, c.t, c.u, xlen[c.b], ylen[c.b] + 1};
+}
+
+// lane 0 of lse_gather: the row's log-softmax denominator (natural order) and its blank / label log-probs (skewed)
+template <typename T, typename X>
+__device__ __forceinline__ void store_lse_logprobs(const RowCell& c, const X* x, T l, int blank, const int* labels,
+                                                   int maxU, long long SK, T* lse, T* lpb, T* lpl) {
+    lse[c.cell] = l;
+    const long long k = c.sk(maxU, SK);
+    lpb[k] = widen(x[blank]) - l;
+    if (c.u < c.Un - 1) lpl[k] = widen(x[c.label(labels, maxU)]) - l;
+}
+
+// Outgoing-arc terms of a valid cell (t,u), gpu_rnnt_kernel.h:163-172; beta points at beta(t,u) in the skewed plane, so
+// beta(t+1,u) = beta[maxU] and beta(t,u+1) = beta[maxU + 1] (next diagonal), each read only where its arc exists:
+//   sb = exp(alpha + lp_blank - ll (+ beta(t+1,u)))    (the last cell's blank arc leaves the lattice: no beta)
+//   sl = exp(alpha + lp_label - ll + beta(t,u+1)),     times (1 + lambda) under FastEmit
+// FastEmit (fe: lambda != 0 and a label arc) also gives lrho = lambda * fastemit_rho (else 0).  Callers combine the
+// terms themselves: their bits depend on the exact expressions.
+template <typename T>
+struct ArcTerms { T sb, sl, lrho; bool fe; };
+template <typename T>
+__device__ __forceinline__ ArcTerms<T> arc_terms(T a, T ll, T lp_blank, T lp_label, const T* beta, int maxU, bool last,
+                                                 bool t_inner, bool has_label, float fastemit_lambda) {
+    ArcTerms<T> r{T(0), T(0), T(0), false};
+    if (last) r.sb = xexp(a + lp_blank - ll);
+    if (t_inner) r.sb = xexp(a + lp_blank - ll + beta[maxU]);
+    if (has_label) r.sl = xexp(a + lp_label - ll + beta[maxU + 1]);
+    if (fastemit_lambda != 0.f && has_label) {
+        const T lam = fastemit_lambda;
+        r.lrho = lam * fastemit_rho<T>(lp_label, beta[maxU + 1], beta[0]);
+        r.sl *= T(1) + lam;
+        r.fe = true;
+    }
+    return r;
+}
+
 // ---------------------------------------------------------------------------------------------
 // lse + gather: one warp per lattice cell (row of V logits).  Row r of `logits` is natural cell
 // row0 + r.  Two in-cache passes (max, then sum exp(x-max)) reproduce the reference's
@@ -167,13 +218,11 @@ __global__ void __launch_bounds__(256) lse_gather_kernel(const X* __restrict__ l
                                                          const int* __restrict__ labels, int maxT, int maxU,
                                                          long long SK, int blank, T* __restrict__ lse,
                                                          T* __restrict__ lpb, T* __restrict__ lpl) {
-    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
-    const long long cell = row0 + row;
-    const CellIdx c = decode_cell(cell, maxT, maxU);
-    const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
-    if (c.t >= Tn || c.u >= Un) return;  // padded cell: never read downstream
+    const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
+    if (c.padded()) return;
     const X* x = logits + row * (long long)V;
     T m = neg_inf<T>();
     for (int v = lane; v < V; v += 32) { T xv = widen(x[v]); m = xv > m ? xv : m; }
@@ -181,13 +230,7 @@ __global__ void __launch_bounds__(256) lse_gather_kernel(const X* __restrict__ l
     T s = 0;
     for (int v = lane; v < V; v += 32) s += xexp(widen(x[v]) - m);
     s = warp_sum(s);
-    if (lane == 0) {
-        const T l = m + xlog(s);
-        lse[cell] = l;
-        const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
-        lpb[k] = widen(x[blank]) - l;
-        if (c.u < Un - 1) lpl[k] = widen(x[labels[(long long)c.b * (maxU - 1) + c.u]]) - l;
-    }
+    if (lane == 0) store_lse_logprobs(c, x, m + xlog(s), blank, labels, maxU, SK, lse, lpb, lpl);
 }
 
 // 16-byte fast path of lse_gather (V a multiple of Vec16<X>::N, 16-byte aligned rows): each lane streams 16-byte pieces
@@ -201,13 +244,11 @@ __global__ void __launch_bounds__(256) lse_gather_vec_kernel(const X* __restrict
                                                              long long SK, int blank, float* __restrict__ lse,
                                                              float* __restrict__ lpb, float* __restrict__ lpl) {
     using P = Vec16<X>;
-    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
-    const long long cell = row0 + row;
-    const CellIdx c = decode_cell(cell, maxT, maxU);
-    const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
-    if (c.t >= Tn || c.u >= Un) return;
+    const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
+    if (c.padded()) return;
     const X* x = logits + row * (long long)V;
     const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
     const int nv = V >> P::LOG2N;
@@ -243,13 +284,7 @@ __global__ void __launch_bounds__(256) lse_gather_vec_kernel(const X* __restrict
         }
     }
     s = warp_sum(s);
-    if (lane == 0) {
-        const float l = m + logf(s);
-        lse[cell] = l;
-        const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
-        lpb[k] = widen(x[blank]) - l;
-        if (c.u < Un - 1) lpl[k] = widen(x[labels[(long long)c.b * (maxU - 1) + c.u]]) - l;
-    }
+    if (lane == 0) store_lse_logprobs(c, x, m + logf(s), blank, labels, maxU, SK, lse, lpb, lpl);
 }
 
 // 16-byte fast path of rnnt_grad_kernel (same arithmetic, 16-byte loads/stores; fp16 / bf16 gradients are rounded once,
@@ -265,35 +300,29 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
                                                             const float* __restrict__ llf,
                                                             const float* __restrict__ gscale, float fastemit_lambda) {
     using P = Vec16<X>;
-    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
-    const long long cell = row0 + row;
-    const CellIdx c = decode_cell(cell, maxT, maxU);
-    const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
+    const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
     const X* x = logits + row * (long long)V;
     const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
     typename P::Raw* gv = reinterpret_cast<typename P::Raw*>(out + row * (long long)V);
     const int nv = V >> P::LOG2N;
-    if (c.t >= Tn || c.u >= Un) {
+    if (c.padded()) {
         const float z[P::N] = {};
         for (int k = lane; k < nv; k += 32) gv[k] = P::narrow(z);
         return;
     }
-    const long long k0 = sk_index(c.b, c.t, c.u, maxU, SK);
-    const float a = alphas[k0], bt = betas[k0], ll = llf[c.b], l = lse[cell];
+    const long long k0 = c.sk(maxU, SK);
+    const float a = alphas[k0], bt = betas[k0], ll = llf[c.b], l = lse[c.cell];
     const float gs = gscale ? gscale[c.b] : 1.f;
-    const int label = (c.u < Un - 1) ? labels[(long long)c.b * (maxU - 1) + c.u] : -1;
-    float sb = 0.f, sl = 0.f;
-    if (c.t == Tn - 1 && c.u == Un - 1) sb = expf(a + (widen(x[blank]) - l) - ll);
-    if (c.t < Tn - 1) sb = expf(a + (widen(x[blank]) - l) - ll + betas[k0 + maxU]);
-    if (label >= 0) sl = expf(a + (widen(x[label]) - l) - ll + betas[k0 + maxU + 1]);
+    const int label = c.label(labels, maxU);
+    const bool last = c.t == c.Tn - 1 && c.u == c.Un - 1, t_inner = c.t < c.Tn - 1;
+    const ArcTerms<float> arc = arc_terms<float>(a, ll, last || t_inner ? widen(x[blank]) - l : 0.f,
+                                                 label >= 0 ? widen(x[label]) - l : 0.f, betas + k0, maxU, last, t_inner,
+                                                 label >= 0, fastemit_lambda);
     float kd = a + bt - ll - l;
-    if (fastemit_lambda != 0.f && label >= 0) {       // FastEmit: see rnnt_grad_kernel
-        const float rho = fastemit_rho(widen(x[label]) - l, betas[k0 + maxU + 1], bt);
-        kd += log1pf(fastemit_lambda * rho);
-        sl *= 1.f + fastemit_lambda;
-    }
+    if (arc.fe) kd += log1pf(arc.lrho);               // FastEmit: see rnnt_grad_kernel
     for (int k = lane; k < nv; k += 32) {
         float v[P::N], g[P::N];
         P::widen(xv[k], v);
@@ -301,7 +330,7 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
         for (int i = 0; i < P::N; ++i) g[i] = expf(v[i] + kd);
         const int db = blank - (k << P::LOG2N), dl = label - (k << P::LOG2N);
 #pragma unroll
-        for (int i = 0; i < P::N; ++i) g[i] -= (db == i ? sb : 0.f) + (dl == i ? sl : 0.f);
+        for (int i = 0; i < P::N; ++i) g[i] -= (db == i ? arc.sb : 0.f) + (dl == i ? arc.sl : 0.f);
 #pragma unroll
         for (int i = 0; i < P::N; ++i) g[i] *= gs;
         gv[k] = P::narrow(g);
@@ -509,7 +538,8 @@ __global__ void __launch_bounds__(BT_THREADS) backtrace_kernel(const unsigned* _
 // FastEmit (fastemit_lambda > 0): the label arc's gradient is scaled by (1 + lambda), so the row becomes
 //   g[v] = (gamma + lambda*gamma_L) p_v - [v==blank] gamma_B - [v==label_u] (1 + lambda) gamma_L,
 // gamma_L = sl; the softmax term is today's times (1 + lambda*rho) (fastemit_rho), i.e. kd += log1p(lambda*rho).
-// lambda == 0 takes none of this arithmetic: the result is bit-identical to the plain loss.
+// arc_terms forms sb, sl and lambda*rho; lambda == 0 takes none of the FastEmit arithmetic: the result is bit-identical
+// to the plain loss.
 // ---------------------------------------------------------------------------------------------
 template <typename T, typename X = T>
 __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out, long long row0, long long nrows,
@@ -520,36 +550,30 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
                                                         const T* __restrict__ alphas, const T* __restrict__ betas,
                                                         const T* __restrict__ llf, const T* __restrict__ gscale,
                                                         float fastemit_lambda) {
-    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
-    const long long cell = row0 + row;
-    const CellIdx c = decode_cell(cell, maxT, maxU);
-    const int Tn = xlen[c.b], Un = ylen[c.b] + 1;
+    const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
     const X* x = logits + row * (long long)V;
     X* g = out + row * (long long)V;
-    if (c.t >= Tn || c.u >= Un) {
+    if (c.padded()) {
         for (int v = lane; v < V; v += 32) g[v] = narrow<X>(T(0));
         return;
     }
-    const long long k = sk_index(c.b, c.t, c.u, maxU, SK);
-    const T a = alphas[k], bt = betas[k], ll = llf[c.b], l = lse[cell];
+    const long long k = c.sk(maxU, SK);
+    const T a = alphas[k], bt = betas[k], ll = llf[c.b], l = lse[c.cell];
     const T gs = gscale ? gscale[c.b] : T(1);
-    const int label = (c.u < Un - 1) ? labels[(long long)c.b * (maxU - 1) + c.u] : -1;
-    T sb = 0, sl = 0;
-    if (c.t == Tn - 1 && c.u == Un - 1) sb = xexp(a + (widen(x[blank]) - l) - ll);
-    if (c.t < Tn - 1) sb = xexp(a + (widen(x[blank]) - l) - ll + betas[k + maxU]);        // beta(t+1,u): next diagonal, same column
-    if (label >= 0) sl = xexp(a + (widen(x[label]) - l) - ll + betas[k + maxU + 1]);      // beta(t,u+1): next diagonal, next column
+    const int label = c.label(labels, maxU);
+    const bool last = c.t == c.Tn - 1 && c.u == c.Un - 1, t_inner = c.t < c.Tn - 1;
+    const ArcTerms<T> arc = arc_terms<T>(a, ll, last || t_inner ? widen(x[blank]) - l : T(0),
+                                         label >= 0 ? widen(x[label]) - l : T(0), betas + k, maxU, last, t_inner,
+                                         label >= 0, fastemit_lambda);
     T kd = a + bt - ll - l;
-    if (fastemit_lambda != 0.f && label >= 0) {
-        const T lam = fastemit_lambda;
-        kd += xlog1p(lam * fastemit_rho<T>(widen(x[label]) - l, betas[k + maxU + 1], bt));
-        sl *= T(1) + lam;
-    }
+    if (arc.fe) kd += xlog1p(arc.lrho);
     for (int v = lane; v < V; v += 32) {
         T gr = xexp(widen(x[v]) + kd);
-        if (v == blank) gr -= sb;
-        if (v == label) gr -= sl;
+        if (v == blank) gr -= arc.sb;
+        if (v == label) gr -= arc.sl;
         g[v] = narrow<X>(gr * gs);
     }
 }
@@ -562,7 +586,8 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
 // values dl_blank, dl_label are formed here from the cached log-probs and stored as E' = dl / rs in place of E, so that
 // rs * E' is exact for them too.  Rows outside the valid lattice get rs = 0 (their E stays finite: it was formed from z = 0).
 // FastEmit (fastemit_lambda > 0, see rnnt_grad_kernel): rs is multiplied by fe = 1 + lambda*rho and the label arc's term
-// by 1 + lambda, which the patched columns absorb; lambda == 0 leaves fe = 1 and every value bit-identical.
+// by 1 + lambda (both from arc_terms), which the patched columns absorb; lambda == 0 leaves fe = 1 and every value
+// bit-identical.
 __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ tile_of_slot, const int* __restrict__ count, int b0,
                                                         int nTb, int nUb, const int* __restrict__ xlen, const int* __restrict__ ylen,
                                                         const int* __restrict__ labels, int blank, int maxT, int maxU, long long SK,
@@ -584,19 +609,15 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
         const long long k = sk_index(b, t, u, maxU, SK);
         const float a = alphas[k], bt = betas[k], ll = llf[b], g = gscale ? gscale[b] : 1.f;
         const float occ = a + bt - ll;                                   // log occupancy of the cell
-        float sb = 0.f, sl_ = 0.f, pl = 0.f;
-        if (t == Tn - 1 && u == Un - 1) sb = expf(a + lpb[k] - ll);
-        if (t < Tn - 1) sb = expf(a + lpb[k] - ll + betas[k + maxU]);
         const bool has_label = u < Un - 1;
-        int lab = -1;
-        if (has_label) { sl_ = expf(a + lpl[k] - ll + betas[k + maxU + 1]); pl = expf(lpl[k] + occ); lab = labels[(long long)b * (maxU - 1) + u]; }
-        float fe = 1.f;                                                  // FastEmit factor of the softmax term
-        if (fastemit_lambda != 0.f && has_label) {
-            fe = 1.f + fastemit_lambda * fastemit_rho(lpl[k], betas[k + maxU + 1], bt);
-            sl_ *= 1.f + fastemit_lambda;
-        }
-        float dlb = g * (fe * expf(lpb[k] + occ) - sb), dll = g * (fe * pl - sl_);
-        if (has_label && lab == blank) { dlb -= g * sl_; dll = dlb; }    // degenerate: label == blank
+        const float lp_label = has_label ? lpl[k] : 0.f;
+        const ArcTerms<float> arc = arc_terms<float>(a, ll, lpb[k], lp_label, betas + k, maxU, t == Tn - 1 && u == Un - 1,
+                                                     t < Tn - 1, has_label, fastemit_lambda);
+        const float pl = has_label ? expf(lp_label + occ) : 0.f;
+        const int lab = has_label ? labels[(long long)b * (maxU - 1) + u] : -1;
+        const float fe = arc.fe ? 1.f + arc.lrho : 1.f;                  // FastEmit factor of the softmax term
+        float dlb = g * (fe * expf(lpb[k] + occ) - arc.sb), dll = g * (fe * pl - arc.sl);
+        if (has_label && lab == blank) { dlb -= g * arc.sl; dll = dlb; } // degenerate: label == blank
         rs = fe * (g * exp2f(rowref[row] + (occ - lse[((long long)b * maxT + t) * maxU + u]) * 1.4426950408889634f));
         // rs is cut to 0 only where 1/rs stops being finite (a denormal rs would make it +inf and the patched columns NaN).
         // The forward keeps lse2 - ref <= FWD_REBASE + log2 V, so a row cut here has |g| * e^occ < 2^-126 * 2^(64 + log2 V):
@@ -630,23 +651,6 @@ __global__ void __launch_bounds__(256) zgen_kernel(const float* __restrict__ enc
         const int h = (int)(i - r * H);
         const CellIdx c = decode_cell(row0 + r, maxT, maxU);
         z[i] = tanhf(enc[((long long)c.b * maxT + c.t) * H + h] + pred[((long long)c.b * maxU + c.u) * H + h]);
-    }
-}
-
-// out[n] += sum_r A[r, n] for a row-major (rows, N) matrix: one block per 32 columns, 8 row lanes, fixed summation order
-__global__ void __launch_bounds__(256) colsum_add_kernel(const float* __restrict__ A, long long rows, int N, float* __restrict__ out) {
-    __shared__ float part[8][33];
-    const int c = threadIdx.x & 31, rl = threadIdx.x >> 5, n = blockIdx.x * 32 + c;
-    float acc = 0.f;
-    if (n < N)
-        for (long long r = rl; r < rows; r += 8) acc += A[r * N + n];
-    part[rl][c] = acc;
-    __syncthreads();
-    if (rl == 0 && n < N) {
-        float s = 0.f;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) s += part[k][c];
-        out[n] += s;
     }
 }
 
@@ -826,7 +830,8 @@ __global__ void __launch_bounds__(256) dz_reduce_kernel(const float* __restrict_
     }
 }
 
-// out[v] += sum_r x[r,v]   (db of the exact path)
+// out[v] += sum_r x[r,v]   (db of the exact path, db1 of dense1): one block per 32 columns and gridDim.y row blocks of 8
+// row lanes.  With gridDim.y == 1 each column has one writer and a fixed summation order: run-to-run deterministic.
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, long long nrows, int V,
                                                      float* __restrict__ out) {
     const int v = blockIdx.x * 32 + (threadIdx.x & 31);

@@ -51,7 +51,7 @@ struct LossWs {
 // (cpu_rnnt.h:166-170: "WARNING: Forward backward likelihood mismatch" when |llForward - llBackward| > 0.1) as a
 // device-side printf: stream-ordered, costs nothing unless it fires, and needs no read-back.
 __global__ void finish_costs_kernel(const float* __restrict__ llf, const float* __restrict__ llb, float* __restrict__ out, int n,
-                                    const int* __restrict__ overflow = nullptr) {
+                                    const int* __restrict__ overflow) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     if (overflow && *overflow) { out[i] = __int_as_float(0x7fc00000); return; }   // broken valid_tile_bound promise (tile_compact_kernel reported it)
@@ -61,6 +61,13 @@ __global__ void finish_costs_kernel(const float* __restrict__ llf, const float* 
 }
 
 inline rnntStatus_t check_launch() { return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED; }
+
+// overflow (nullable): the tensor-core forward's broken valid_tile_bound word, which turns the costs into NaN
+rnntStatus_t launch_finish_costs(const float* llf, const float* llb, float* costs, int B, const int* overflow, cudaStream_t s) {
+    finish_costs_kernel<<<(B + 127) / 128, 128, 0, s>>>(llf, llb, costs, B, overflow);
+    RB_LAUNCHED(1);
+    return check_launch();
+}
 
 template <typename T>
 rnntStatus_t launch_alpha_beta(const LossWs<T>& w, const int* xlen, const int* ylen, int B, int maxT, int maxU,
@@ -162,24 +169,35 @@ rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, co
     return check_launch();
 }
 
-// loss op on materialised logits: lse+gather -> alpha/beta -> (grad).  costs stay on device in w.llf.
-template <typename T>
-rnntStatus_t loss_op(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, const T* gscale,
-                     int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s, float fastemit_lambda) {
-    const bool vec = vec_ok<T>(acts, grads, V);
-    rnntStatus_t st = loss_planes<T, T>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s);
-    if (st || !grads) return st;
-    return loss_grads<T, T>(acts, grads, vec, labels, ylen, xlen, gscale, V, B, maxT, maxU, blank, workspace, s,
-                            fastemit_lambda);
+// forward of the device-costs entries (fp32 or 16-bit logits over a float workspace): planes, then the costs
+template <typename X>
+rnntStatus_t loss_forward(const X* acts, bool vec, const int* labels, const int* ylen, const int* xlen, int V, int B,
+                          int maxT, int maxU, int blank, float* costs, void* workspace, cudaStream_t s) {
+    rnntStatus_t st = loss_planes<float, X>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s);
+    if (st) return st;
+    const LossWs<float> w(workspace, B, maxT, maxU);
+    return launch_finish_costs(w.llf, w.llb, costs, B, nullptr, s);
+}
+
+// argument checks of rnnt_entrypoint.cpp:49-60, shared by the loss-op entries (out: the costs, or the 16-bit gradients)
+bool loss_args_ok(const void* acts, const int* labels, const int* ylen, const int* xlen, int V, int B, const void* out,
+                  const void* workspace, const rnntOptions& o) {
+    return acts && labels && ylen && xlen && out && workspace && V > 0 && B > 0 && o.maxT > 0 && o.maxU > 0;
 }
 
 // argument checks of the 16-bit entries (those of rnntb200_loss_device, plus the logit type, the blank index and the
 // wavefront's maxU bound, so that the backward rejects what its forward would have)
 bool loss16_args_ok(const void* acts, int logit_type, const int* labels, const int* ylen, const int* xlen, int V, int B,
                     const void* out, const void* workspace, const rnntOptions& o) {
-    return acts && labels && ylen && xlen && out && workspace && V > 0 && B > 0 && o.maxT > 0 && o.maxU > 0 &&
-           o.maxU <= 1024 && o.blank_label >= 0 && o.blank_label < V &&
-           (logit_type == RNNTB200_LOGITS_F16 || logit_type == RNNTB200_LOGITS_BF16);
+    return loss_args_ok(acts, labels, ylen, xlen, V, B, out, workspace, o) && o.maxU <= 1024 && o.blank_label >= 0 &&
+           o.blank_label < V && (logit_type == RNNTB200_LOGITS_F16 || logit_type == RNNTB200_LOGITS_BF16);
+}
+
+// f(logits, gradients) with the pointers typed by the 16-bit logit type (loss16_args_ok has checked it)
+template <typename F>
+rnntStatus_t with_logits16(int logit_type, const void* acts, void* grads, F&& f) {
+    if (logit_type == RNNTB200_LOGITS_F16) return f(static_cast<const __half*>(acts), static_cast<__half*>(grads));
+    return f(static_cast<const __nv_bfloat16*>(acts), static_cast<__nv_bfloat16*>(grads));
 }
 
 // FastEmit's lambda: finite and >= 0 (NaN fails both comparisons)
@@ -188,18 +206,18 @@ inline bool fastemit_ok(float lambda) { return lambda >= 0.f && lambda <= FLT_MA
 template <typename T>
 rnntStatus_t compute_impl(const T* acts, T* grads, const int* labels, const int* ylen, const int* xlen, int V, int B,
                           T* costs_host, void* workspace, rnntOptions opt) {
-    // argument checks of rnnt_entrypoint.cpp:49-60
-    if (!acts || !labels || !ylen || !xlen || !costs_host || !workspace || V <= 0 || B <= 0 || opt.maxT <= 0 ||
-        opt.maxU <= 0)
-        return RNNT_STATUS_INVALID_VALUE;
+    if (!loss_args_ok(acts, labels, ylen, xlen, V, B, costs_host, workspace, opt)) return RNNT_STATUS_INVALID_VALUE;
     if (opt.loc == RNNT_CPU) {
         fprintf(stderr, "rnnt_b200: RNNT_CPU requested but this library has no CPU path (no fallback by design)\n");
         return RNNT_STATUS_EXECUTION_FAILED;
     }
     if (opt.loc != RNNT_GPU) return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(opt.stream);
-    rnntStatus_t st = loss_op<T>(acts, grads, labels, ylen, xlen, nullptr, V, B, opt.maxT, opt.maxU, opt.blank_label,
-                                 workspace, s, 0.f);
+    const bool vec = vec_ok<T>(acts, grads, V);
+    rnntStatus_t st = loss_planes<T, T>(acts, vec, labels, ylen, xlen, V, B, opt.maxT, opt.maxU, opt.blank_label, workspace, s);
+    if (!st && grads)
+        st = loss_grads<T, T>(acts, grads, vec, labels, ylen, xlen, nullptr, V, B, opt.maxT, opt.maxU, opt.blank_label,
+                              workspace, s, 0.f);
     if (st) return st;
     // costs to HOST + sync + negate, as gpu_rnnt.h:209-213; llBackward comes along for the guard of cpu_rnnt.h:166-170
     LossWs<T> w(workspace, B, opt.maxT, opt.maxU);
@@ -237,11 +255,10 @@ struct JointWs {
             chunk_rows = (long long)ch;
             scratch_bytes = ch * per_row;
         } else {
-#ifndef RNNTB200_NO_TC
             chunk_rows = 0;
+#ifndef RNNTB200_NO_TC
             scratch_bytes = rb::tc_scratch_bytes(d);
 #else
-            chunk_rows = 0;
             scratch_bytes = 0;
 #endif
         }
@@ -286,10 +303,13 @@ void launch_sgemm(const float* A, const float* Bm, float* C, const float* bias, 
     }
     RB_LAUNCHED(1);
 }
-void launch_sgemm_zw(const float* Z, const float* W, const float* bias, float* L, long long rows, int H, int V,
-                     cudaStream_t s) {
+// Rows r0 .. r0+rows of the exact path's projection: Z = tanh(enc + pred) (model.py:158-163), then L = Z.W + b
+void exact_project(const rnntb200JointDesc& d, const float* enc, const float* pred, const float* W, const float* bias,
+                   long long r0, long long rows, float* Z, float* L, cudaStream_t s) {
+    rb::zgen_kernel<<<ew_blocks(rows * d.H), 256, 0, s>>>(enc, pred, Z, r0, rows, d.maxT, d.maxU, d.H);
+    RB_LAUNCHED(1);
     rb::ScopedTimer tm("sgemm L=Z.W+b", s);
-    launch_sgemm<true, true>(Z, W, L, bias, (int)rows, V, H, H, 1, V, 1, V, 0, s);
+    launch_sgemm<true, true>(Z, W, L, bias, (int)rows, d.V, d.H, d.H, 1, d.V, 1, d.V, 0, s);
 }
 
 rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
@@ -300,9 +320,7 @@ rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const 
     float* L = Z + ws.chunk_rows * d.H;
     for (long long r0 = 0; r0 < N; r0 += ws.chunk_rows) {
         const long long rows = (N - r0 < ws.chunk_rows) ? N - r0 : ws.chunk_rows;
-        rb::zgen_kernel<<<ew_blocks(rows * d.H), 256, 0, s>>>(enc, pred, Z, r0, rows, d.maxT, d.maxU, d.H);
-        RB_LAUNCHED(1);
-        launch_sgemm_zw(Z, W, bias, L, rows, d.H, d.V, s);
+        exact_project(d, enc, pred, W, bias, r0, rows, Z, L, s);
         rb::lse_gather_kernel<float><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
             L, r0, rows, d.V, xlen, ylen, labels, d.maxT, d.maxU, SK, d.blank_label, ws.loss.lse, ws.loss.lpb,
             ws.loss.lpl);
@@ -327,8 +345,7 @@ rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const
         return RNNT_STATUS_MEMOPS_FAILED;
     for (long long r0 = 0; r0 < N; r0 += ws.chunk_rows) {
         const long long rows = (N - r0 < ws.chunk_rows) ? N - r0 : ws.chunk_rows;
-        rb::zgen_kernel<<<ew_blocks(rows * d.H), 256, 0, s>>>(enc, pred, Z, r0, rows, d.maxT, d.maxU, d.H);
-        launch_sgemm_zw(Z, W, bias, L, rows, d.H, d.V, s);
+        exact_project(d, enc, pred, W, bias, r0, rows, Z, L, s);
         // dlogits in place (gpu_rnnt_kernel.h:143-179 formula, times the upstream per-utterance gradient)
         rb::rnnt_grad_kernel<float><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
             L, L, r0, rows, d.V, xlen, ylen, labels, d.maxT, d.maxU, SK, d.blank_label, ws.loss.lse, ws.loss.alphas,
@@ -350,10 +367,54 @@ rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const
             if (gy > 512) gy = 512;
             rb::colsum_kernel<<<dim3((d.V + 31) / 32, (unsigned)gy), 256, 0, s>>>(L, rows, d.V, db);
         }
-        RB_LAUNCHED(5);
+        RB_LAUNCHED(4);
         if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
     }
     return RNNT_STATUS_SUCCESS;
+}
+
+#ifdef RNNTB200_NO_TC
+inline rnntStatus_t tc_missing() {
+    fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
+    return RNNT_STATUS_EXECUTION_FAILED;
+}
+#endif
+
+// The joint forward of the loss and alignment entries: projection (exact or tensor-core), alpha/beta, costs.  *overflow:
+// the broken-valid_tile_bound word finish_costs reads (nullptr: none).  A keeping forward has just ranked the tiles, so
+// its word is fresh; one that keeps nothing counts them only for the alignment (check_bound).
+rnntStatus_t joint_forward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
+                           const float* W, const float* bias, const int* labels, const int* ylen, const int* xlen,
+                           float* costs, bool check_bound, const int** overflow, cudaStream_t s) {
+    *overflow = nullptr;
+    rnntStatus_t st;
+    if (d.precision == RNNTB200_FP32_EXACT) {
+        st = exact_forward(d, ws, enc, pred, W, bias, labels, ylen, xlen, s);
+    } else {
+#ifndef RNNTB200_NO_TC
+        unsigned nl = 0;
+        st = rb::tc_forward(d, ws.scratch, enc, pred, W, bias, labels, ylen, xlen, ws.loss.lse, ws.loss.lpb, ws.loss.lpl,
+                            s, &nl);
+        if (!st) {
+            const rb::TcScratch sc = rb::tc_scratch_layout(d, ws.scratch);
+            if (check_bound) *overflow = rb::tc_check_tile_bound(d, ws.scratch, ylen, xlen, s, &nl);
+            else if (rb::tc_keep(d, sc)) *overflow = sc.count + 1;
+        }
+        RB_LAUNCHED(nl);
+#else
+        st = tc_missing();
+#endif
+    }
+    if (st) return st;
+    st = launch_alpha_beta(ws.loss, xlen, ylen, d.B, d.maxT, d.maxU, s);
+    if (st) return st;
+    return launch_finish_costs(ws.loss.llf, ws.loss.llb, costs, d.B, *overflow, s);
+}
+
+// argument checks shared by the joint entries that run the loss (forward, backward, alignment)
+bool joint_loss_args_ok(const rnntb200JointDesc* d, const float* enc, const float* pred, const float* W,
+                        const float* bias, const int* labels, const int* ylen, const int* xlen, const void* workspace) {
+    return desc_ok(d) && enc && pred && W && bias && labels && ylen && xlen && workspace;
 }
 
 }  // namespace
@@ -411,18 +472,17 @@ rnntStatus_t rnntb200_loss_device_fastemit(const float* activations, float* grad
                                            const int* label_lengths, const int* input_lengths, const float* grad_scale,
                                            int alphabet_size, int minibatch, float* costs_device, void* workspace,
                                            rnntOptions options, float fastemit_lambda) {
-    if (!activations || !flat_labels || !label_lengths || !input_lengths || !costs_device || !workspace ||
-        alphabet_size <= 0 || minibatch <= 0 || options.maxT <= 0 || options.maxU <= 0 || !fastemit_ok(fastemit_lambda))
+    if (!loss_args_ok(activations, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch, costs_device,
+                      workspace, options) || !fastemit_ok(fastemit_lambda))
         return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
-    rnntStatus_t st = loss_op<float>(activations, gradients, flat_labels, label_lengths, input_lengths, grad_scale,
-                                     alphabet_size, minibatch, options.maxT, options.maxU, options.blank_label,
-                                     workspace, s, fastemit_lambda);
-    if (st) return st;
-    LossWs<float> w(workspace, minibatch, options.maxT, options.maxU);
-    finish_costs_kernel<<<(minibatch + 127) / 128, 128, 0, s>>>(w.llf, w.llb, costs_device, minibatch);
-    RB_LAUNCHED(1);
-    return check_launch();
+    const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
+    const bool vec = vec_ok<float>(activations, gradients, V);
+    rnntStatus_t st = loss_forward(activations, vec, flat_labels, label_lengths, input_lengths, V, B, T, U, blank,
+                                   costs_device, workspace, s);
+    if (st || !gradients) return st;
+    return loss_grads<float, float>(activations, gradients, vec, flat_labels, label_lengths, input_lengths, grad_scale, V,
+                                    B, T, U, blank, workspace, s, fastemit_lambda);
 }
 
 rnntStatus_t rnntb200_loss16_forward(const void* activations, int logit_type, const int* flat_labels,
@@ -433,21 +493,10 @@ rnntStatus_t rnntb200_loss16_forward(const void* activations, int logit_type, co
         return RNNT_STATUS_INVALID_VALUE;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
-    rnntStatus_t st;
-    if (logit_type == RNNTB200_LOGITS_F16) {
-        const __half* x = static_cast<const __half*>(activations);
-        st = loss_planes<float, __half>(x, vec_ok<float, __half>(x, nullptr, V), flat_labels, label_lengths, input_lengths,
-                                        V, B, T, U, blank, workspace, s);
-    } else {
-        const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(activations);
-        st = loss_planes<float, __nv_bfloat16>(x, vec_ok<float, __nv_bfloat16>(x, nullptr, V), flat_labels, label_lengths,
-                                               input_lengths, V, B, T, U, blank, workspace, s);
-    }
-    if (st) return st;
-    LossWs<float> w(workspace, B, T, U);
-    finish_costs_kernel<<<(B + 127) / 128, 128, 0, s>>>(w.llf, w.llb, costs_device, B);
-    RB_LAUNCHED(1);
-    return check_launch();
+    return with_logits16(logit_type, activations, nullptr, [&](auto x, auto g) {
+        return loss_forward(x, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, V, B, T, U, blank,
+                            costs_device, workspace, s);
+    });
 }
 
 rnntStatus_t rnntb200_loss16_backward(const void* activations, int logit_type, const int* flat_labels,
@@ -468,16 +517,10 @@ rnntStatus_t rnntb200_loss16_backward_fastemit(const void* activations, int logi
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
     void* ws = const_cast<void*>(workspace);      // read only: LossWs just carves the planes out of it
-    if (logit_type == RNNTB200_LOGITS_F16) {
-        const __half* x = static_cast<const __half*>(activations);
-        __half* g = static_cast<__half*>(gradients);
-        return loss_grads<float, __half>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, grad_costs,
-                                         V, B, T, U, blank, ws, s, fastemit_lambda);
-    }
-    const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(activations);
-    __nv_bfloat16* g = static_cast<__nv_bfloat16*>(gradients);
-    return loss_grads<float, __nv_bfloat16>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths,
-                                            grad_costs, V, B, T, U, blank, ws, s, fastemit_lambda);
+    return with_logits16(logit_type, activations, gradients, [&](auto x, auto g) {
+        return loss_grads<float>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, grad_costs, V, B,
+                                 T, U, blank, ws, s, fastemit_lambda);
+    });
 }
 
 rnntStatus_t rnntb200_joint_workspace_size(const rnntb200JointDesc* desc, size_t* size_bytes) {
@@ -491,39 +534,11 @@ rnntStatus_t rnntb200_joint_loss_forward(const rnntb200JointDesc* desc, const fl
                                          const float* W, const float* bias, const int* labels,
                                          const int* label_lengths, const int* input_lengths, float* costs,
                                          void* workspace) {
-    if (!desc_ok(desc) || !enc || !pred || !W || !bias || !labels || !label_lengths || !input_lengths || !costs ||
-        !workspace)
+    if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !costs)
         return RNNT_STATUS_INVALID_VALUE;
-    const rnntb200JointDesc& d = *desc;
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
-    JointWs ws(d, workspace);
-    rnntStatus_t st;
-    if (d.precision == RNNTB200_FP32_EXACT) {
-        st = exact_forward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, s);
-    } else {
-#ifndef RNNTB200_NO_TC
-        unsigned nl = 0;
-        st = rb::tc_forward(d, ws.scratch, enc, pred, W, bias, labels, label_lengths, input_lengths, ws.loss.lse,
-                            ws.loss.lpb, ws.loss.lpl, s, &nl);
-        RB_LAUNCHED(nl);
-#else
-        fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
-        st = RNNT_STATUS_EXECUTION_FAILED;
-#endif
-    }
-    if (st) return st;
-    st = launch_alpha_beta(ws.loss, input_lengths, label_lengths, d.B, d.maxT, d.maxU, s);
-    if (st) return st;
-    const int* overflow = nullptr;
-#ifndef RNNTB200_NO_TC
-    if (d.precision != RNNTB200_FP32_EXACT) {      // the keeping forward ranked the tiles: its overflow word is fresh
-        const rb::TcScratch sc = rb::tc_scratch_layout(d, ws.scratch);
-        if (rb::tc_keep(d, sc)) overflow = sc.count + 1;
-    }
-#endif
-    finish_costs_kernel<<<(d.B + 127) / 128, 128, 0, s>>>(ws.loss.llf, ws.loss.llb, costs, d.B, overflow);
-    RB_LAUNCHED(1);
-    return check_launch();
+    const int* overflow;
+    return joint_forward(*desc, JointWs(*desc, workspace), enc, pred, W, bias, labels, label_lengths, input_lengths, costs,
+                         false, &overflow, reinterpret_cast<cudaStream_t>(desc->stream));
 }
 
 rnntStatus_t rnntb200_joint_loss_backward(const rnntb200JointDesc* desc, const float* enc, const float* pred,
@@ -540,8 +555,8 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
                                                    const int* label_lengths, const int* input_lengths,
                                                    const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                                    float* db, void* workspace, float fastemit_lambda) {
-    if (!desc_ok(desc) || !enc || !pred || !W || !bias || !labels || !label_lengths || !input_lengths ||
-        !grad_costs || !d_enc || !d_pred || !dW || !db || !workspace || !fastemit_ok(fastemit_lambda))
+    if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !grad_costs ||
+        !d_enc || !d_pred || !dW || !db || !fastemit_ok(fastemit_lambda))
         return RNNT_STATUS_INVALID_VALUE;
     const rnntb200JointDesc& d = *desc;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
@@ -557,8 +572,7 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
     RB_LAUNCHED(nl);
     return st;
 #else
-    fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
-    return RNNT_STATUS_EXECUTION_FAILED;
+    return tc_missing();
 #endif
 }
 
@@ -592,35 +606,16 @@ rnntStatus_t rnntb200_joint_align(const rnntb200JointDesc* desc, const float* en
                                   const float* bias, const int* labels, const int* label_lengths,
                                   const int* input_lengths, float* costs, float* best_logp, int* label_frames,
                                   void* workspace) {
-    if (!desc_ok(desc) || !enc || !pred || !W || !bias || !labels || !label_lengths || !input_lengths || !costs ||
-        !workspace || !align_args_ok(best_logp, label_frames, desc->maxU))
+    if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !costs ||
+        !align_args_ok(best_logp, label_frames, desc->maxU))
         return RNNT_STATUS_INVALID_VALUE;
     rnntb200JointDesc d = *desc;
     d.keep_activations = 0;                 // no backward follows: nothing beyond the loss planes is kept
     cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
     JointWs ws(d, workspace);
-    const int* overflow = nullptr;
-    rnntStatus_t st;
-    if (d.precision == RNNTB200_FP32_EXACT) {
-        st = exact_forward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, s);
-    } else {
-#ifndef RNNTB200_NO_TC
-        unsigned nl = 0;
-        st = rb::tc_forward(d, ws.scratch, enc, pred, W, bias, labels, label_lengths, input_lengths, ws.loss.lse,
-                            ws.loss.lpb, ws.loss.lpl, s, &nl);
-        if (!st) overflow = rb::tc_check_tile_bound(d, ws.scratch, label_lengths, input_lengths, s, &nl);
-        RB_LAUNCHED(nl);
-#else
-        fprintf(stderr, "rnnt_b200: built without the tensor-core path\n");
-        st = RNNT_STATUS_EXECUTION_FAILED;
-#endif
-    }
+    const int* overflow;
+    rnntStatus_t st = joint_forward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, costs, true, &overflow, s);
     if (st) return st;
-    st = launch_alpha_beta(ws.loss, input_lengths, label_lengths, d.B, d.maxT, d.maxU, s);
-    if (st) return st;
-    finish_costs_kernel<<<(d.B + 127) / 128, 128, 0, s>>>(ws.loss.llf, ws.loss.llb, costs, d.B, overflow);
-    RB_LAUNCHED(1);
-    if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
     return launch_align(ws.loss, input_lengths, label_lengths, d.B, d.maxT, d.maxU, overflow, best_logp, label_frames, s);
 }
 
@@ -632,12 +627,9 @@ rnntStatus_t rnntb200_joint_logits(const rnntb200JointDesc* desc, const float* e
     cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
     JointWs ws(d, workspace);
     const long long N = (long long)d.B * d.maxT * d.maxU;
-    float* Z = reinterpret_cast<float*>(ws.scratch);
     for (long long r0 = 0; r0 < N; r0 += ws.chunk_rows) {
         const long long rows = (N - r0 < ws.chunk_rows) ? N - r0 : ws.chunk_rows;
-        rb::zgen_kernel<<<ew_blocks(rows * d.H), 256, 0, s>>>(enc, pred, Z, r0, rows, d.maxT, d.maxU, d.H);
-        launch_sgemm_zw(Z, W, bias, logits + r0 * d.V, rows, d.H, d.V, s);
-        RB_LAUNCHED(1);
+        exact_project(d, enc, pred, W, bias, r0, rows, reinterpret_cast<float*>(ws.scratch), logits + r0 * d.V, s);
         if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
     }
     return RNNT_STATUS_SUCCESS;
@@ -685,7 +677,7 @@ rnntStatus_t rnntb200_dense1_backward(const float* X, const float* dA, const flo
     }
     if (db1) {
         rb::ScopedTimer tm("dense1 db1+=colsum(dA)", s);
-        rb::colsum_add_kernel<<<(H + 31) / 32, 256, 0, s>>>(dA, rows, H, db1);
+        rb::colsum_kernel<<<dim3((H + 31) / 32, 1), 256, 0, s>>>(dA, rows, H, db1);      // one row block: deterministic
         RB_LAUNCHED(1);
     }
     return check_launch();

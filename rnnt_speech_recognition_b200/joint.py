@@ -22,9 +22,7 @@ __all__ = ["joint_rnnt_loss", "joint_logits", "joint_step", "Joint", "get_fused_
 
 _PREC = {"fp32": _lib.FP32_EXACT, "bf16": _lib.BF16_TC, _lib.FP32_EXACT: _lib.FP32_EXACT, _lib.BF16_TC: _lib.BF16_TC}
 
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
+_ptr = _lib.ptr
 
 
 def valid_tile_count(input_lengths, label_lengths):
@@ -36,8 +34,8 @@ def valid_tile_count(input_lengths, label_lengths):
 
 def _desc(B, T, U, H, V, blank, precision, keep=False, tile_bound=0):
     # (call inside `with torch.cuda.device(...)`: the stream is the CURRENT stream of the tensors' device)
-    return _lib.JointDesc(B, T, U, H, V, int(blank), _PREC[precision],
-                          C.c_void_p(torch.cuda.current_stream().cuda_stream).value, int(tile_bound or 0), 1 if keep else 0)
+    return _lib.JointDesc(B, T, U, H, V, int(blank), _PREC[precision], _lib.stream().value, int(tile_bound or 0),
+                          1 if keep else 0)
 
 
 def _workspace(desc, device):
@@ -76,42 +74,49 @@ def _check(enc, pred, W, b, labels, input_lengths, label_lengths):
         raise ValueError("must have a length per example.")
 
 
+def _joint_setup(enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, keep, valid_tiles):
+    """What the joint loss and alignment calls do before their call: contiguous operands and their checks, a 1-element
+    stand-in for labels with no elements (U == 1), the descriptor and its workspace.  Returns the operands in the order
+    of the C entries (enc, pred, W, b, labels, label_lengths, input_lengths), the descriptor and the workspace."""
+    enc, pred, W, b = (t.contiguous() for t in (enc, pred, W, b))
+    labels, input_lengths, label_lengths = (t.contiguous() for t in (labels, input_lengths, label_lengths))
+    _check(enc, pred, W, b, labels, input_lengths, label_lengths)
+    B, T, H = enc.shape
+    U, V = pred.shape[1], W.shape[1]
+    lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=enc.device)
+    with torch.cuda.device(enc.device):
+        desc = _desc(B, T, U, H, V, blank, precision, keep, valid_tiles)
+    return (enc, pred, W, b, lab, label_lengths, input_lengths), desc, _workspace(desc, enc.device)
+
+
 class _JointRNNT(torch.autograd.Function):
     @staticmethod
     def forward(ctx, enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, compact, keep=None, valid_tiles=None,
                 fastemit_lambda=0.0):
         L = _lib.load()
-        enc, pred, W, b = (t.contiguous() for t in (enc, pred, W, b))
-        labels, input_lengths, label_lengths = (t.contiguous() for t in (labels, input_lengths, label_lengths))
-        _check(enc, pred, W, b, labels, input_lengths, label_lengths)
-        B, T, H = enc.shape
-        U, V = pred.shape[1], W.shape[1]
-        lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=enc.device)
-        with torch.cuda.device(enc.device):
-            # a backward will follow: let the forward keep its softmax numerators / tanh outputs in the workspace
-            keep = any(ctx.needs_input_grad[:4]) if keep is None else bool(keep)
-            desc = _desc(B, T, U, H, V, blank, precision, keep, valid_tiles)
-            ws = _workspace(desc, enc.device)
-            costs = torch.empty(B, dtype=torch.float32, device=enc.device)
-            st = L.rnntb200_joint_loss_forward(C.byref(desc), _ptr(enc), _ptr(pred), _ptr(W), _ptr(b), _ptr(lab),
-                                               _ptr(label_lengths), _ptr(input_lengths), _ptr(costs), _ptr(ws))
+        # a backward will follow: let the forward keep its softmax numerators / tanh outputs in the workspace
+        keep = any(ctx.needs_input_grad[:4]) if keep is None else keep
+        args, desc, ws = _joint_setup(enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, keep,
+                                      valid_tiles)
+        device = args[0].device
+        costs = torch.empty(desc.B, dtype=torch.float32, device=device)
+        with torch.cuda.device(device):
+            st = L.rnntb200_joint_loss_forward(C.byref(desc), *map(_ptr, args), _ptr(costs), _ptr(ws))
         _lib.check(st, "rnntb200_joint_loss_forward")
-        ctx.save_for_backward(enc, pred, W, b, lab, input_lengths, label_lengths)
-        ctx.ws, ctx.dims, ctx.blank, ctx.precision, ctx.compact, ctx.keep = ws, (B, T, U, H, V), blank, precision, compact, keep
-        ctx.valid_tiles, ctx.fastemit_lambda = valid_tiles, fastemit_lambda
+        ctx.save_for_backward(*args)
+        ctx.ws, ctx.desc, ctx.fastemit_lambda = ws, desc, fastemit_lambda
         return costs
 
     @staticmethod
     def backward(ctx, grad_costs):
         L = _lib.load()
-        enc, pred, W, b, lab, input_lengths, label_lengths = ctx.saved_tensors
-        B, T, U, H, V = ctx.dims
+        args = ctx.saved_tensors
         g = grad_costs.to(torch.float32).contiguous()
-        d_enc, d_pred, dW, db = (torch.empty_like(t) for t in (enc, pred, W, b))
-        with torch.cuda.device(enc.device):
-            desc = _desc(B, T, U, H, V, ctx.blank, ctx.precision, ctx.keep, ctx.valid_tiles)
-            st = L.rnntb200_joint_loss_backward_fastemit(C.byref(desc), _ptr(enc), _ptr(pred), _ptr(W), _ptr(b), _ptr(lab),
-                                                         _ptr(label_lengths), _ptr(input_lengths), _ptr(g), _ptr(d_enc),
+        d_enc, d_pred, dW, db = (torch.empty_like(t) for t in args[:4])
+        with torch.cuda.device(args[0].device):
+            desc = ctx.desc
+            desc.stream = _lib.stream().value          # the forward's descriptor, on the backward's current stream
+            st = L.rnntb200_joint_loss_backward_fastemit(C.byref(desc), *map(_ptr, args), _ptr(g), _ptr(d_enc),
                                                          _ptr(d_pred), _ptr(dW), _ptr(db), _ptr(ctx.ws), ctx.fastemit_lambda)
         _lib.check(st, "rnntb200_joint_loss_backward_fastemit")
         ctx.ws = None
@@ -183,7 +188,7 @@ def joint_step(f, g, K1, b1, K2, b2, want_logits=True, want_best=False):
         logp = torch.empty(B, dtype=torch.float32, device=f.device) if want_best else None
         st = L.rnntb200_joint_step(_ptr(f.detach()), f.stride(0), _ptr(g.detach()), g.stride(0), _ptr(K1c), _ptr(b1c), _ptr(K2c),
                                    _ptr(b2c), B, P, H, V, _ptr(logits), _ptr(best), _ptr(logp),
-                                   C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                   _lib.stream())
     _lib.check(st, "rnntb200_joint_step")
     return logits, best, logp
 
@@ -206,7 +211,7 @@ class _Dense1(torch.autograd.Function):
         with torch.cuda.device(x.device):
             out = torch.empty(*x.shape[:-1], H, dtype=torch.float32, device=x.device)
             st = L.rnntb200_dense1_forward(_ptr(xc), rows, P, _ptr(Kc), _ptr(bc), H, _ptr(out),
-                                           C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                           _lib.stream())
         _lib.check(st, "rnntb200_dense1_forward")
         ctx.save_for_backward(xc, Kc)
         ctx.has_bias = b1 is not None
@@ -225,7 +230,7 @@ class _Dense1(torch.autograd.Function):
             dK = torch.zeros_like(Kc) if need_k else None          # the entry accumulates
             db = torch.zeros(H, dtype=torch.float32, device=xc.device) if need_b else None
             st = L.rnntb200_dense1_backward(_ptr(xc), _ptr(dA), _ptr(Kc), rows, P, H, _ptr(dX), _ptr(dK), _ptr(db),
-                                            C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                            _lib.stream())
         _lib.check(st, "rnntb200_dense1_backward")
         return dX, dK, db
 

@@ -27,13 +27,7 @@ from . import _lib
 
 __all__ = ["rnnt_loss", "torch_rnnt_loss", "RNNTLoss", "certify_inputs"]
 
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+_ptr = _lib.ptr
 
 
 def check_type(var, t, name):
@@ -80,15 +74,32 @@ def certify_inputs(log_probs, labels, lengths, label_lengths, check_max=True):
             raise ValueError("Output length mismatch")
 
 
-def _require_cuda(t, name):
-    if not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor: rnnt_b200 has no CPU path (no fallback by design)" % name)
-
-
 def workspace_bytes(maxT, maxU, B, dtype_size=4):
     sz = C.c_size_t(0)
     _lib.check(_lib.load().get_workspace_size(maxT, maxU, B, True, C.byref(sz), dtype_size), "get_workspace_size")
     return sz.value
+
+
+def _prepare(acts, labels, act_lens, label_lens, float32_only=False):
+    """The checks and buffers of every call on materialised logits: all tensors on the device, (for the float32-only op,
+    warprnnt_op.cc:15) float32 logits, labels (B, U-1); then the loss workspace, and a 1-element stand-in for labels
+    with no elements (U == 1).  Returns (B, T, U, V), workspace, labels."""
+    for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
+        if not t.is_cuda:
+            raise RuntimeError("%s must be a CUDA tensor: rnnt_b200 has no CPU path (no fallback by design)" % n)
+    if float32_only and acts.dtype != torch.float32:
+        raise TypeError("acts must be torch.float32")
+    B, T, U, V = acts.shape
+    if labels.shape[1] != U - 1 and not (U == 1 and labels.shape[1] == 0):
+        raise ValueError("labels must be (B, U-1)")
+    ws = torch.empty(workspace_bytes(T, U, B), dtype=torch.uint8, device=acts.device)
+    lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
+    return (B, T, U, V), ws, lab
+
+
+def _options(blank, T, U):
+    # (call inside `with torch.cuda.device(...)`: the stream must be the current stream OF THE TENSORS' DEVICE)
+    return _lib.RnntOptions(_lib.RNNT_GPU, 0, _lib.stream().value, int(blank), T, U, True)
 
 
 class _RNNTOp(torch.autograd.Function):
@@ -98,22 +109,13 @@ class _RNNTOp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
         L = _lib.load()
-        for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
-            _require_cuda(t, n)
-        if acts.dtype != torch.float32:
-            raise TypeError("acts must be torch.float32")      # op registered float32-only, warprnnt_op.cc:15
-        B, T, U, V = acts.shape
-        if labels.shape[1] != U - 1 and not (U == 1 and labels.shape[1] == 0):
-            raise ValueError("labels must be (B, U-1)")
-        need_grad = acts.requires_grad
-        grads = torch.empty_like(acts) if need_grad else None
+        (B, T, U, V), ws, lab = _prepare(acts, labels, act_lens, label_lens, float32_only=True)
+        grads = torch.empty_like(acts) if acts.requires_grad else None
         costs = torch.empty(B, dtype=torch.float32, device=acts.device)
-        ws = torch.empty(workspace_bytes(T, U, B), dtype=torch.uint8, device=acts.device)
-        lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
-        with torch.cuda.device(acts.device):     # the stream must be the current stream OF THE TENSORS' DEVICE
-            opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, int(blank), T, U, True)
+        with torch.cuda.device(acts.device):
             st = L.rnntb200_loss_device_fastemit(_ptr(acts), _ptr(grads), _ptr(lab), _ptr(label_lens), _ptr(act_lens),
-                                                 None, V, B, _ptr(costs), _ptr(ws), opt, fastemit_lambda)
+                                                 None, V, B, _ptr(costs), _ptr(ws), _options(blank, T, U),
+                                                 fastemit_lambda)
         _lib.check(st, "rnntb200_loss_device_fastemit")
         ctx.grads = grads
         return costs
@@ -136,18 +138,11 @@ class _RNNTOp16(torch.autograd.Function):
     @staticmethod
     def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
         L = _lib.load()
-        for t, n in ((acts, "acts"), (labels, "labels"), (act_lens, "input_lengths"), (label_lens, "label_lengths")):
-            _require_cuda(t, n)
-        B, T, U, V = acts.shape
-        if labels.shape[1] != U - 1 and not (U == 1 and labels.shape[1] == 0):
-            raise ValueError("labels must be (B, U-1)")
+        (B, T, U, V), ws, lab = _prepare(acts, labels, act_lens, label_lens)
         costs = torch.empty(B, dtype=torch.float32, device=acts.device)
-        ws = torch.empty(workspace_bytes(T, U, B), dtype=torch.uint8, device=acts.device)
-        lab = labels if labels.numel() else torch.zeros(1, dtype=torch.int32, device=acts.device)
         with torch.cuda.device(acts.device):
-            opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, int(blank), T, U, True)
             st = L.rnntb200_loss16_forward(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
-                                           _ptr(act_lens), V, B, _ptr(costs), _ptr(ws), opt)
+                                           _ptr(act_lens), V, B, _ptr(costs), _ptr(ws), _options(blank, T, U))
         _lib.check(st, "rnntb200_loss16_forward")
         if acts.requires_grad:
             ctx.save_for_backward(acts, lab, act_lens, label_lens)
@@ -163,10 +158,9 @@ class _RNNTOp16(torch.autograd.Function):
         g = grad_costs.to(torch.float32).contiguous()
         grads = torch.empty_like(acts)
         with torch.cuda.device(acts.device):
-            opt = _lib.RnntOptions(_lib.RNNT_GPU, 0, _stream().value, ctx.blank, T, U, True)
             st = L.rnntb200_loss16_backward_fastemit(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
-                                                     _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws), opt,
-                                                     ctx.fastemit_lambda)
+                                                     _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws),
+                                                     _options(ctx.blank, T, U), ctx.fastemit_lambda)
         _lib.check(st, "rnntb200_loss16_backward_fastemit")
         ctx.ws = None
         return grads, None, None, None, None, None
