@@ -6,7 +6,8 @@
 // two 2-byte writes per row).  A scale per ROW commutes with both GEMMs, so neither needs a per-element prologue:
 //
 //   bwd_dz_kernel   dZ[rows,H] = rs_row * (E'[rows,V] . W^T): both operands straight from TMA (K-major), then the row
-//                   scale, (1 - tanh^2(enc+pred)) and the tile's sums over u (-> d_enc, accumulated in shared memory along
+//                   scale, (1 - tanh^2(enc+pred)) (enc / pred rows staged in shared memory by TMA) and the tile's sums
+//                   over u (-> d_enc, accumulated in shared memory along
 //                   a run of tiles and stored once) and over t (-> one fp32 partial plane of d_pred per t-block).
 //                   Neither dl nor dZ ever exists in HBM.
 //   bwd_dw_kernel   [dW; db][H+1,V] (+)= ([rs_row * z, rs_row])^T . E'  as a split-K GEMM over the lattice rows: the A operand
@@ -28,6 +29,7 @@ constexpr int BWD_THREADS = 288;        // dZ: warps 0-3 / 4-7: consumer warpgro
 constexpr int DZ_NC = 128;              // h columns per dZ pass (m64n128 accumulators)
 constexpr int DZ_GS_LD = DZ_NC + 8;     // row stride (floats) of the staged gradient tile
 constexpr int DZ_MAX_STAGES = 4;
+constexpr int DZ_IN_ENC = 0, DZ_IN_PRED = 16 * DZ_NC * 4, DZ_IN_BYTES = DZ_IN_PRED + 8 * DZ_NC * 4;   // a pass's enc / pred slice
 constexpr int DW_NV = 128;              // vocabulary columns per dW output tile
 constexpr int DW_STAGES = 4;            // K steps in flight between the producers and the MMA warpgroups (A + B per stage)
 
@@ -56,24 +58,35 @@ struct BwdParams {
 // Work order (identical in both roles): runs = (utterance, t-block) assigned round-robin to CTAs; inside a run the valid
 // tiles along u; inside a tile ceil(H / 128) passes of 128 columns (the last pass of an H % 128 == 64 model reads W rows
 // past H as TMA zero fill and stores nothing for them).  A stage = the tile's E' block [128 rows x 64 v] + the pass's W
-// rows [128 h x 64 v].
+// rows [128 h x 64 v].  Besides the ring, one input slot holds the pass's enc rows [16 t x 128 h] and pred rows
+// [8 u x 128 h] (fp32 boxes, rows past the arrays read as 0) for the epilogue: the TMA lane loads it halfway through the
+// pass's K blocks, by when the previous pass's epilogue has released it, so the epilogue finds its inputs in shared
+// memory instead of waiting on global loads.
 __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_constant__ CUtensorMap tmap_e,
                                                                 const __grid_constant__ CUtensorMap tmap_w,
+                                                                const __grid_constant__ CUtensorMap tmap_enc,
+                                                                const __grid_constant__ CUtensorMap tmap_pred,
                                                                 const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const int KBV = p.V >> 6, NPASS = (p.H + DZ_NC - 1) / DZ_NC, stages = p.dz_stages;
     float* gs = reinterpret_cast<float*>(smem + (size_t)stages * 32768);      // [128][DZ_GS_LD] staged gradient rows
     float* dacc = gs + 128 * DZ_GS_LD;                                          // [16][H] the run's d_enc rows
-    uint64_t* full = reinterpret_cast<uint64_t*>(dacc + 16 * p.H);
+    uint8_t* inp = reinterpret_cast<uint8_t*>(dacc + 16 * p.H);                // the pass's enc / pred slice
+    uint64_t* full = reinterpret_cast<uint64_t*>(inp + DZ_IN_BYTES);
     uint64_t* empty = full + DZ_MAX_STAGES;
+    uint64_t* in_full = empty + DZ_MAX_STAGES;
+    uint64_t* in_empty = in_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int i = 0; i < DZ_MAX_STAGES; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 2); }
+        ptx::mbar_init(in_full, 1); ptx::mbar_init(in_empty, 1);
         ptx::fence_barrier_init();
     }
-    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_w); }
+    if (warp == 8 && lane == 0) {
+        ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_enc); ptx::prefetch_tmap(&tmap_pred);
+    }
     for (int i = threadIdx.x; i < 16 * p.H; i += BWD_THREADS) dacc[i] = 0.f;
     __syncthreads();
     const int nruns = p.nb * p.nTb;
@@ -81,7 +94,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
     if (warp == 8) {
         // ===================== TMA: A = kept numerators [128 rows x 64 v], B = W rows [128 h x 64 v] =====================
         if (lane == 0) {
-            int st = 0; uint32_t ph = 0;
+            int st = 0; uint32_t ph = 0, iph = 0;
             for (int run = blockIdx.x; run < nruns; run += gridDim.x) {
                 const int bl = run / p.nTb, tb = run - bl * p.nTb, b = p.b0 + bl;
                 const int Tn = p.xlen[b], Un = p.ylen[b] + 1;
@@ -92,6 +105,13 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                     const int sl = max(p.slot ? p.slot[tile] : tile, 0);   // a slot-less tile (broken bound) has rs = 0 everywhere
                     for (int pass = 0; pass < NPASS; ++pass)
                         for (int kb = 0; kb < KBV; ++kb) {
+                            if (kb == KBV / 2) {
+                                ptx::mbar_wait(in_empty, iph ^ 1);
+                                ptx::mbar_arrive_expect_tx(in_full, (uint32_t)DZ_IN_BYTES);
+                                ptx::tma_load_2d(inp + DZ_IN_ENC, &tmap_enc, in_full, pass * DZ_NC, b * p.maxT + tb * BW_TT);
+                                ptx::tma_load_2d(inp + DZ_IN_PRED, &tmap_pred, in_full, pass * DZ_NC, b * p.maxU + ub * BW_UU);
+                                iph ^= 1;
+                            }
                             ptx::mbar_wait(&empty[st], ph ^ 1);
                             ptx::mbar_arrive_expect_tx(&full[st], 32768u);
                             uint8_t* sa = smem + (size_t)st * 32768;
@@ -108,8 +128,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
     // ===================== consumer warpgroups: D[64 x 128] += A[64 x 64] . B[128 x 64]^T, then the epilogue =====================
     const int wg = threadIdx.x >> 7, t128 = threadIdx.x & 127, q = lane & 3;
     const int Ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);          // rows Ra and Ra + 8 of the tile
-    const uint32_t s_a = ptx::smem_u32(smem);
-    int st = 0; uint32_t ph = 0;
+    const uint32_t s_a = ptx::smem_u32(smem), in_a = ptx::smem_u32(inp);
+    int st = 0; uint32_t ph = 0, iph = 0;
     for (int run = blockIdx.x; run < nruns; run += gridDim.x) {
         const int bl = run / p.nTb, tb = run - bl * p.nTb, b = p.b0 + bl;
         const int Tn = p.xlen[b], Un = p.ylen[b] + 1;
@@ -119,15 +139,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
             const int tile = (bl * p.nTb + tb) * p.nUb + ub;
             const int tslot = p.slot ? p.slot[tile] : tile;               // < 0 only after a broken valid_tile_bound promise
             float rs[2];
-            const float* erow[2];
-            const float* prow[2];
 #pragma unroll
-            for (int ri = 0; ri < 2; ++ri) {
-                const int r = Ra + 8 * ri, t = tb * BW_TT + (r >> 3), u = ub * BW_UU + (r & 7);
-                rs[ri] = tslot >= 0 ? __ldg(p.rowscale + (size_t)tslot * 128 + r) : 0.f;   // 0 outside the lattice
-                erow[ri] = p.enc + ((size_t)b * p.maxT + min(t, p.maxT - 1)) * p.H;
-                prow[ri] = p.pred + ((size_t)b * p.maxU + min(u, p.maxU - 1)) * p.H;
-            }
+            for (int ri = 0; ri < 2; ++ri)      // 0 outside the lattice
+                rs[ri] = tslot >= 0 ? __ldg(p.rowscale + (size_t)tslot * 128 + Ra + 8 * ri) : 0.f;
             for (int pass = 0; pass < NPASS; ++pass) {
                 const int n0 = pass * DZ_NC;
                 float acc[64];
@@ -151,16 +165,20 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                 if (t128 == 0) ptx::mbar_arrive(&empty[prev]);
                 ptx::fence_regs(acc);
                 // ---- g = rs * acc * (1 - tanh^2(enc + pred)) -> staged tile
+                ptx::mbar_wait(in_full, iph);
+                iph ^= 1;
 #pragma unroll
                 for (int ri = 0; ri < 2; ++ri) {
-                    float* grow = gs + (Ra + 8 * ri) * DZ_GS_LD + 2 * q;
+                    const int r = Ra + 8 * ri;
+                    float* grow = gs + r * DZ_GS_LD + 2 * q;
+                    const uint32_t erow = in_a + DZ_IN_ENC + (uint32_t)((r >> 3) * DZ_NC + 2 * q) * 4u,
+                                   prow = in_a + DZ_IN_PRED + (uint32_t)((r & 7) * DZ_NC + 2 * q) * 4u;
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const int h = n0 + 8 * j + 2 * q;
                         float2 g = make_float2(0.f, 0.f);
                         if (rs[ri] != 0.f && h < p.H) {
-                            const float2 e = __ldg(reinterpret_cast<const float2*>(erow[ri] + h)),
-                                         pq = __ldg(reinterpret_cast<const float2*>(prow[ri] + h));
+                            const float2 e = ptx::lds64f(erow + 32u * j), pq = ptx::lds64f(prow + 32u * j);
                             const float z0 = ptx::tanh_approx(e.x + pq.x), z1 = ptx::tanh_approx(e.y + pq.y);
                             const float d0 = acc[4 * j + 2 * ri] * rs[ri], d1 = acc[4 * j + 2 * ri + 1] * rs[ri];
                             g = make_float2(fmaf(-d0 * z0, z0, d0), fmaf(-d1 * z1, z1, d1));
@@ -169,22 +187,32 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                     }
                 }
                 ptx::named_bar_sync(1, 256);
-                // ---- sums over u (into the run's d_enc rows) and over t (this t-block's d_pred plane), fixed order
-                for (int i = threadIdx.x; i < 16 * DZ_NC; i += 256) {
-                    const int tl = i / DZ_NC, col = i - tl * DZ_NC;
+                if (threadIdx.x == 0) ptx::mbar_arrive(in_empty);      // the input slot has been read
+                // ---- sums over u (into the run's d_enc rows) and over t (this t-block's d_pred plane), fixed order, four
+                //      columns per thread
+                for (int i = threadIdx.x; i < 16 * DZ_NC / 4; i += 256) {
+                    const int tl = i / (DZ_NC / 4), col = 4 * (i - tl * (DZ_NC / 4));
                     if (n0 + col >= p.H) continue;
-                    float sum = 0.f;
+                    float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-                    for (int ul = 0; ul < BW_UU; ++ul) sum += gs[(tl * 8 + ul) * DZ_GS_LD + col];
-                    dacc[tl * p.H + n0 + col] += sum;
+                    for (int ul = 0; ul < BW_UU; ++ul) {
+                        const float4 v = *reinterpret_cast<const float4*>(gs + (tl * 8 + ul) * DZ_GS_LD + col);
+                        sum.x += v.x; sum.y += v.y; sum.z += v.z; sum.w += v.w;
+                    }
+                    float4* d = reinterpret_cast<float4*>(dacc + tl * p.H + n0 + col);
+                    const float4 a = *d;
+                    *d = make_float4(a.x + sum.x, a.y + sum.y, a.z + sum.z, a.w + sum.w);
                 }
-                for (int i = threadIdx.x; i < BW_UU * DZ_NC; i += 256) {
-                    const int ul = i / DZ_NC, col = i - ul * DZ_NC, u = ub * BW_UU + ul;
+                for (int i = threadIdx.x; i < BW_UU * DZ_NC / 4; i += 256) {
+                    const int ul = i / (DZ_NC / 4), col = 4 * (i - ul * (DZ_NC / 4)), u = ub * BW_UU + ul;
                     if (n0 + col >= p.H || u >= p.maxU) continue;
-                    float sum = 0.f;
+                    float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-                    for (int tl = 0; tl < BW_TT; ++tl) sum += gs[(tl * 8 + ul) * DZ_GS_LD + col];
-                    p.ppred[(((size_t)tb * p.nb + bl) * p.maxU + u) * p.H + n0 + col] = sum;
+                    for (int tl = 0; tl < BW_TT; ++tl) {
+                        const float4 v = *reinterpret_cast<const float4*>(gs + (tl * 8 + ul) * DZ_GS_LD + col);
+                        sum.x += v.x; sum.y += v.y; sum.z += v.z; sum.w += v.w;
+                    }
+                    *reinterpret_cast<float4*>(p.ppred + (((size_t)tb * p.nb + bl) * p.maxU + u) * p.H + n0 + col) = sum;
                 }
                 ptx::named_bar_sync(1, 256);
             }
@@ -201,7 +229,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
 struct DzGeom { int stages; size_t smem_bytes; bool ok; };
 inline DzGeom dz_geometry(int H) {
     DzGeom g{};
-    const size_t fixed = 1024 + (size_t)128 * DZ_GS_LD * 4 + (size_t)16 * H * 4 + 2 * DZ_MAX_STAGES * 8;
+    const size_t fixed = 1024 + (size_t)128 * DZ_GS_LD * 4 + (size_t)16 * H * 4 + DZ_IN_BYTES + (2 * DZ_MAX_STAGES + 2) * 8;
     g.stages = fixed < TC_SMEM_OPTIN ? (int)((TC_SMEM_OPTIN - fixed) / 32768) : 0;
     if (g.stages > DZ_MAX_STAGES) g.stages = DZ_MAX_STAGES;
     g.smem_bytes = fixed + (size_t)g.stages * 32768;

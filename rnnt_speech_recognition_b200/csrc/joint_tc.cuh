@@ -441,7 +441,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         {
             const int nruns = nb * g.nTb;
             ScopedTimer tmr("bwd_dz_kernel", s);
-            bwd_dz_kernel<<<nruns < sms ? nruns : sms, BWD_THREADS, zg.smem_bytes, s>>>(tm_e128, tm_w, p);
+            bwd_dz_kernel<<<nruns < sms ? nruns : sms, BWD_THREADS, zg.smem_bytes, s>>>(tm_e128, tm_w, tm_enc, tm_pred, p);
         }
         {
             const size_t n4 = (size_t)nb * d.maxU * d.H / 4;
