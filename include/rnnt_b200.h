@@ -289,7 +289,12 @@ rnntStatus_t rnntb200_joint_logits(const rnntb200JointDesc* desc, const float* e
  *  in ONE launch (thread-block clusters of 8 CTAs per row; fp32 FMA arithmetic).  f, g: (B,P) device rows with strides
  *  ldf, ldg (so f = encoded[:, i, :] and g = pred_out[:, -1, :] need no copy); K1 (P,H) and b1 (H) are Keras Dense-1
  *  (K1 == NULL: f, g are the already projected activations, P == H); K2 (H,V), b2 (V).  Any of logits (B,V), best (B),
- *  best_logp (B) may be NULL, not all.  P <= 4096, H <= 2048. */
+ *  best_logp (B) may be NULL, not all.
+ *  Non-finite logits: a NaN outranks every number and the first NaN wins (as np.argmax / torch.argmax), so best[b] always
+ *  lies in [0, V) -- 0 for a row of -inf.  best_logp[b] is NaN for a row that holds a NaN or only -inf.
+ *  Limits: P <= 4096, H <= 2048 and V <= 8 * (58088 - max(P, 256) - H - 256): each CTA holds its eighth of the logits in
+ *  shared memory, 4 * (max(P, 256) + H + 256 + ceil(V / 8)) bytes within the 227 KB per block of sm_90 (V <= 460096 at
+ *  P = H = 64, 413504 at P = 4096, H = 2048).  Past them: RNNT_STATUS_INVALID_VALUE before any device work. */
 rnntStatus_t rnntb200_joint_step(const float* f, long long ldf, const float* g, long long ldg, const float* K1,
                                  const float* b1, const float* K2, const float* b2, int B, int P, int H, int V,
                                  float* logits, int* best, float* best_logp, CUstream stream);
@@ -301,7 +306,9 @@ rnntStatus_t rnntb200_joint_step(const float* f, long long ldf, const float* g, 
  *    backward:  dX = dA . K1^T;  dK1 += X^T . dA;  db1 += sum_r dA[r,:]      (dX, dK1, db1 may each be NULL; dK1 / db1 are
  *               ACCUMULATED into, so the encoder-side and the prediction-side call add into one zeroed buffer)
  *  fp32 FMA kernels of this library (no GEMM library).  dK1 is a split-K product combined with float atomics: its last bits
- *  depend on the order the partial sums arrive in (as the exact fp32 path's dW). */
+ *  depend on the order the partial sums arrive in (as the exact fp32 path's dW).  1 <= rows <= INT_MAX (X may exceed 2^31
+ *  elements; a product taller than one launch's 65535 row tiles runs as several launches), else
+ *  RNNT_STATUS_INVALID_VALUE, as for dX without K1 and dK1 without X. */
 rnntStatus_t rnntb200_dense1_forward(const float* X, long long rows, int P, const float* K1, const float* b1, int H,
                                      float* out, CUstream stream);
 rnntStatus_t rnntb200_dense1_backward(const float* X, const float* dA, const float* K1, long long rows, int P, int H,

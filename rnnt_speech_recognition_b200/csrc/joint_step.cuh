@@ -19,6 +19,18 @@ namespace rb {
 constexpr int STEP_CLUSTER = 8;
 constexpr int STEP_THREADS = 256;
 constexpr int STEP_MAX_DIM = 4096;     // P, H <= 4096 (shared-memory staging of the input row and the hidden row)
+// Shared memory per CTA: the static part_m / part_s / part_i below plus the dynamic joint_step_smem().  Together they may
+// reach 48 KB by default and the sm_90 opt-in ceiling of 227 KB with cudaFuncAttributeMaxDynamicSharedMemorySize.
+constexpr size_t STEP_STATIC_SMEM = STEP_CLUSTER * (2 * sizeof(float) + sizeof(int));
+constexpr size_t STEP_SMEM_DEFAULT = 48 * 1024 - STEP_STATIC_SMEM;    // largest dynamic size without the opt-in
+constexpr size_t STEP_SMEM_MAX = 232448 - STEP_STATIC_SMEM;           // largest dynamic size with it
+
+// Argmax order of the decode step: a NaN outranks every number (the first NaN wins, as np.argmax / torch.argmax), and
+// among equal values the smaller index wins (as tf.argmax).  Is (c, ic) ahead of (a, ia)?
+__device__ __forceinline__ bool step_argmax_before(float c, int ic, float a, int ia) {
+    if (c != c) return a == a || ic < ia;
+    return c > a || (c == a && ic < ia);
+}
 
 struct StepParams {
     const float* f; const float* g;     // (B, P) rows with strides ldf / ldg
@@ -104,10 +116,13 @@ __global__ void __cluster_dims__(STEP_CLUSTER, 1, 1) __launch_bounds__(STEP_THRE
         }
     }
     __syncthreads();
-    // slice max / argmax (smallest index among equal maxima, as tf.argmax), then sum of exp against the slice max
+    // slice max / argmax in the order of step_argmax_before, then sum of exp against the slice max.  Each thread starts
+    // from its first element, so a slice of -inf still yields one of its indices; (-inf, INT_MAX) stands for a thread
+    // (or CTA) that owns no element and loses to every element.
     float my = -CUDART_INF_F; int myi = 0x7fffffff;
-    for (int i = tid; i < vn; i += STEP_THREADS)
-        if (lg[i] > my) { my = lg[i]; myi = v0 + i; }       // ascending index per thread: the first maximum is kept
+    if (tid < vn) { my = lg[tid]; myi = v0 + tid; }
+    for (int i = tid + STEP_THREADS; i < vn; i += STEP_THREADS)
+        if (step_argmax_before(lg[i], v0 + i, my, myi)) { my = lg[i]; myi = v0 + i; }
     int* redi = reinterpret_cast<int*>(x);                  // (the input row is dead: reuse it; P >= 1 ... see launcher: smem has room)
     red[tid] = my; redi[tid] = myi;
     __syncthreads();
@@ -115,15 +130,16 @@ __global__ void __cluster_dims__(STEP_CLUSTER, 1, 1) __launch_bounds__(STEP_THRE
         if (tid < o) {
             const float a2 = red[tid], c2 = red[tid + o];
             const int ia = redi[tid], ic = redi[tid + o];
-            if (c2 > a2 || (c2 == a2 && ic < ia)) { red[tid] = c2; redi[tid] = ic; }
+            if (step_argmax_before(c2, ic, a2, ia)) { red[tid] = c2; redi[tid] = ic; }
         }
         __syncthreads();
     }
     const float bm = red[0];
     const int bi = redi[0];
     __syncthreads();
-    float ssum = 0.f;
-    for (int i = tid; i < vn; i += STEP_THREADS) ssum += expf(lg[i] - bm);
+    float ssum = 0.f;                                       // (a slice of -inf adds nothing: not exp(-inf - -inf) = NaN)
+    if (bm != -CUDART_INF_F)
+        for (int i = tid; i < vn; i += STEP_THREADS) ssum += expf(lg[i] - bm);
     red[tid] = ssum;
     __syncthreads();
     for (int o = STEP_THREADS / 2; o > 0; o >>= 1) {
@@ -141,7 +157,7 @@ __global__ void __cluster_dims__(STEP_CLUSTER, 1, 1) __launch_bounds__(STEP_THRE
     if (rank == 0 && tid == 0) {
         float M = -CUDART_INF_F; int I = 0x7fffffff;
         for (int r = 0; r < STEP_CLUSTER; ++r)
-            if (part_m[r] > M || (part_m[r] == M && part_i[r] < I)) { M = part_m[r]; I = part_i[r]; }
+            if (step_argmax_before(part_m[r], part_i[r], M, I)) { M = part_m[r]; I = part_i[r]; }
         float S = 0.f;
         for (int r = 0; r < STEP_CLUSTER; ++r) S += part_s[r] * expf(part_m[r] - M);
         if (p.best) p.best[b] = I;
@@ -154,6 +170,12 @@ inline size_t joint_step_smem(int P, int H, int V) {
     const int vs = (V + STEP_CLUSTER - 1) / STEP_CLUSTER;
     const int xs = P > STEP_THREADS ? P : STEP_THREADS;      // the input row is reused as the int scratch of the argmax
     return sizeof(float) * ((size_t)xs + H + STEP_THREADS + vs);
+}
+
+// Largest V whose joint_step_smem() fits STEP_SMEM_MAX (P, H within their limits): 8 (58088 - max(P,256) - H - 256).
+inline int joint_step_max_v(int P, int H) {
+    const int xs = P > STEP_THREADS ? P : STEP_THREADS;
+    return STEP_CLUSTER * ((int)(STEP_SMEM_MAX / sizeof(float)) - xs - H - STEP_THREADS);
 }
 
 }  // namespace rb

@@ -249,7 +249,7 @@ inline rnntStatus_t tc_unsupported(const rnntb200JointDesc& d) {
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-DEVICE property of a kernel: set it once per (device, kernel),
 // thread-safe (the library may be driven from several host threads / several devices of one process).
-inline bool tc_smem_optin(const void* func) {
+inline bool tc_smem_optin(const void* func, size_t bytes = TC_SMEM_OPTIN) {
     static std::mutex mu;
     static std::unordered_map<unsigned long long, bool> done;
     int dev = 0;
@@ -258,7 +258,10 @@ inline bool tc_smem_optin(const void* func) {
     std::lock_guard<std::mutex> lk(mu);
     auto it = done.find(key);
     if (it != done.end()) return true;
-    if (cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_OPTIN) != cudaSuccess) return false;
+    if (cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) {
+        cudaGetLastError();         // reported by the caller's status: not left pending for the next call's launch check
+        return false;
+    }
     done[key] = true;
     return true;
 }

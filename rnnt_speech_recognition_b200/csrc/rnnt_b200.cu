@@ -277,7 +277,9 @@ inline unsigned ew_blocks(long long total) {
     return (unsigned)(b > 132 * 32 ? 132 * 32 : (b < 1 ? 1 : b));
 }
 
-// C[M,N] (+)= A.B with generic strides; picks the 128x128 float4 kernel when alignment allows
+// C[M,N] (+)= A.B with generic strides; picks the 128x128 float4 kernel when alignment allows.  The row tiles go in
+// gridDim.y, which holds at most 65535 of them: a taller product runs as one launch per 65535 row tiles, each on the
+// rows m0 .. m0+mc of A and C (A + m0*sAm, C + m0*ldc; 128-row steps keep the fast kernel's 16-byte alignment).
 template <bool AK, bool BN_>
 void launch_sgemm(const float* A, const float* Bm, float* C, const float* bias, int M, int N, int K, long long sAm,
                   long long sAk, long long sBk, long long sBn, long long ldc, int accumulate, cudaStream_t s) {
@@ -285,23 +287,29 @@ void launch_sgemm(const float* A, const float* Bm, float* C, const float* bias, 
     const bool a_ok = AK ? (K % 4 == 0 && sAm % 4 == 0) : (M % 4 == 0 && sAk % 4 == 0);
     const bool b_ok = BN_ ? (N % 4 == 0 && sBk % 4 == 0) : (K % 4 == 0 && sBn % 4 == 0);
     const bool fast = a_ok && b_ok && N % 4 == 0 && ldc % 4 == 0 && al16(A) && al16(Bm) && al16(C) && (!bias || al16(bias));
-    if (fast) {
-        // few output tiles but a long K (dW = Z^T.dL): split K over blockIdx.z so the grid fills the 132 SMs;
-        // only for accumulating calls, whose output already holds valid data to atomically add into
-        int splits = 1;
-        const int tiles = ((N + 127) / 128) * ((M + 127) / 128);
-        if (accumulate && tiles < 132 && K >= 4096) {
-            splits = (132 * 4 + tiles - 1) / tiles;
-            if (splits > K / 512) splits = K / 512;
-            if (splits < 1) splits = 1;
+    const long long mstep = 65535LL * (fast ? 128 : 64);
+    for (long long m0 = 0; m0 < M; m0 += mstep) {
+        const int mc = (int)(M - m0 < mstep ? M - m0 : mstep);
+        const float* Am = A + m0 * sAm;
+        float* Cm = C + m0 * ldc;
+        if (fast) {
+            // few output tiles but a long K (dW = Z^T.dL): split K over blockIdx.z so the grid fills the 132 SMs;
+            // only for accumulating calls, whose output already holds valid data to atomically add into
+            int splits = 1;
+            const int tiles = ((N + 127) / 128) * ((mc + 127) / 128);
+            if (accumulate && tiles < 132 && K >= 4096) {
+                splits = (132 * 4 + tiles - 1) / tiles;
+                if (splits > K / 512) splits = K / 512;
+                if (splits < 1) splits = 1;
+            }
+            dim3 grid((N + 127) / 128, (unsigned)((mc + 127) / 128), splits);
+            rb::sgemm128_kernel<AK, BN_><<<grid, 256, 0, s>>>(Am, Bm, Cm, bias, mc, N, K, sAm, sAk, sBk, sBn, ldc, accumulate);
+        } else {
+            dim3 grid((N + 63) / 64, (unsigned)((mc + 63) / 64));
+            rb::sgemm_kernel<AK, BN_><<<grid, 256, 0, s>>>(Am, Bm, Cm, bias, mc, N, K, sAm, sAk, sBk, sBn, ldc, accumulate);
         }
-        dim3 grid((N + 127) / 128, (unsigned)((M + 127) / 128), splits);
-        rb::sgemm128_kernel<AK, BN_><<<grid, 256, 0, s>>>(A, Bm, C, bias, M, N, K, sAm, sAk, sBk, sBn, ldc, accumulate);
-    } else {
-        dim3 grid((N + 63) / 64, (unsigned)((M + 63) / 64));
-        rb::sgemm_kernel<AK, BN_><<<grid, 256, 0, s>>>(A, Bm, C, bias, M, N, K, sAm, sAk, sBk, sBn, ldc, accumulate);
+        RB_LAUNCHED(1);
     }
-    RB_LAUNCHED(1);
 }
 // Rows r0 .. r0+rows of the exact path's projection: Z = tanh(enc + pred) (model.py:158-163), then L = Z.W + b
 void exact_project(const rnntb200JointDesc& d, const float* enc, const float* pred, const float* W, const float* bias,
@@ -640,13 +648,19 @@ rnntStatus_t rnntb200_joint_step(const float* f, long long ldf, const float* g, 
                                  float* logits, int* best, float* best_logp, CUstream stream) {
     if (!f || !g || !K2 || B <= 0 || P <= 0 || H <= 0 || V <= 0 || (!logits && !best && !best_logp)) return RNNT_STATUS_INVALID_VALUE;
     if (!K1 && P != H) return RNNT_STATUS_INVALID_VALUE;
-    if (P > rb::STEP_MAX_DIM || H > rb::STEP_CLUSTER * rb::STEP_THREADS || V > (1 << 20)) {
+    if (P > rb::STEP_MAX_DIM || H > rb::STEP_CLUSTER * rb::STEP_THREADS) {
         fprintf(stderr, "rnnt_b200: rnntb200_joint_step supports P <= %d, H <= %d\n", rb::STEP_MAX_DIM, rb::STEP_CLUSTER * rb::STEP_THREADS);
+        return RNNT_STATUS_INVALID_VALUE;
+    }
+    if (V > rb::joint_step_max_v(P, H)) {     // each CTA keeps its eighth of the logits in shared memory
+        fprintf(stderr, "rnnt_b200: rnntb200_joint_step supports V <= %d at P = %d, H = %d\n", rb::joint_step_max_v(P, H), P, H);
         return RNNT_STATUS_INVALID_VALUE;
     }
     rb::StepParams p{f, g, ldf, ldg, K1, b1, K2, b2, B, P, H, V, logits, best, best_logp};
     const size_t smem = rb::joint_step_smem(P, H, V);
-    if (smem > 48 * 1024 && !rb::tc_smem_optin(reinterpret_cast<const void*>(rb::joint_step_kernel))) return RNNT_STATUS_EXECUTION_FAILED;
+    if (smem > rb::STEP_SMEM_DEFAULT &&
+        !rb::tc_smem_optin(reinterpret_cast<const void*>(rb::joint_step_kernel), rb::STEP_SMEM_MAX))
+        return RNNT_STATUS_EXECUTION_FAILED;
     rb::joint_step_kernel<<<B * rb::STEP_CLUSTER, rb::STEP_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     RB_LAUNCHED(1);
     return check_launch();
