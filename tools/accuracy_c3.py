@@ -1,36 +1,56 @@
-"""Measured error of the bf16 tensor-core path against the fp32 exact CUDA path at the benchmark configuration
-(BASELINE C3 by default): costs and all four gradients.  `python tools/accuracy_c3.py [B T U V H]`"""
+"""Measured error of the bf16 tensor-core path and of the fp32 exact path against the chunked float64 reference
+(tests/joint_ref64.py) at the benchmark configuration: costs and all four gradients, one JSON line per path.
+
+  python tools/accuracy_c3.py                 # BASELINE C3 (bench.py's inputs, seed 1234)
+  python tools/accuracy_c3.py c5              # BASELINE C5 (bf16 with valid_tiles, as bench.py runs it)
+  python tools/accuracy_c3.py B T U V H       # another dense shape
+"""
 import json
 import os
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import rnnt_speech_recognition_b200 as rb
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+import bench  # noqa: E402
+import joint_ref64 as r64  # noqa: E402
+import rnnt_speech_recognition_b200 as rb  # noqa: E402
 
-B, T, U, V, H = [int(x) for x in sys.argv[1:6]] if len(sys.argv) >= 6 else (32, 512, 128, 1024, 640)
-g = torch.Generator().manual_seed(1234)
-enc, pred = torch.randn(B, T, H, generator=g).cuda(), torch.randn(B, U, H, generator=g).cuda()
-W, b = (torch.randn(H, V, generator=g) / H ** 0.5).cuda(), torch.zeros(V).cuda()
-lab = torch.randint(1, V, (B, U - 1), generator=g, dtype=torch.int32).cuda()
-il = torch.full((B,), T, dtype=torch.int32).cuda()
-ll = torch.full((B,), U - 1, dtype=torch.int32).cuda()
+if len(sys.argv) >= 6:
+    B, T, U, V, H = (int(x) for x in sys.argv[1:6])
+    name, cfg = "custom", dict(B=B, T=T, U=U, V=V, H=H)
+else:
+    name = sys.argv[1] if len(sys.argv) > 1 else "c3"
+    cfg = bench.WORKLOADS[name]
+d = bench.synth(cfg, 1234, "cuda")
+enc, pred, W, b, lab, il, ll = (d[n] for n in ("enc", "pred", "W", "b", "labels", "il", "ll"))
+B = enc.shape[0]
+vt = rb.valid_tile_count(il.tolist(), ll.tolist()) if cfg.get("ragged") else None
+
+want = r64.joint_loss_grad(enc, pred, W, b, lab, il, ll, grad_scale=[1.0 / B] * B)
+torch.cuda.empty_cache()
 
 
 def run(prec):
     t = [x.clone().requires_grad_() for x in (enc, pred, W, b)]
-    costs = rb.joint_rnnt_loss(*t, lab, il, ll, precision=prec)
+    costs = rb.joint_rnnt_loss(*t, lab, il, ll, precision=prec, valid_tiles=vt if prec == "bf16" else None)
     (costs.sum() / B).backward()
     torch.cuda.synchronize()
-    return costs.detach().double(), [x.grad.double() for x in t]
+    out = costs.detach().double().cpu(), [x.grad.double().cpu() for x in t]
+    del t, costs
+    torch.cuda.empty_cache()
+    return out
 
 
-c32, g32 = run("fp32")
-c16, g16 = run("bf16")
-out = {"config": [B, T, U, V, H], "cost_mean": c32.mean().item(),
-       "cost_max_rel_err": ((c16 - c32).abs() / c32.abs()).max().item()}
-for n, a, r in zip(("d_enc", "d_pred", "dW", "db"), g16, g32):
-    out[n] = {"rel_frobenius": ((a - r).norm() / r.norm()).item(), "max_abs_err": (a - r).abs().max().item(),
-              "max_abs_ref": r.abs().max().item()}
-print(json.dumps(out))
+ref_costs = torch.as_tensor(want["costs"])
+for prec in ("bf16", "fp32"):
+    c, g = run(prec)
+    out = {"config": name, "shape": [cfg[k] for k in "BTUVH"], "path": prec, "reference": "float64",
+           "device": torch.cuda.get_device_name(), "cost_max": ref_costs.abs().max().item(),
+           "cost_max_rel_err": ((c - ref_costs).abs() / ref_costs.abs()).max().item()}
+    for n, a in zip(("d_enc", "d_pred", "dW", "db"), g):
+        r = torch.as_tensor(want[n])
+        out[n] = {"rel_frobenius": ((a - r).norm() / r.norm()).item(),
+                  "max_abs_err_over_max": ((a - r).abs().max() / r.abs().max()).item()}
+    print(json.dumps(out))
