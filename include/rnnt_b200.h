@@ -197,7 +197,7 @@ typedef struct {
     CUstream stream;
     /** 0: unknown.  N > 0: the caller promises that at most N of the batch's 16 x 8 lattice tiles intersect the valid lattice,
      *  N >= sum_b ceil(T_b / 16) * ceil((U_b + 1) / 8) with U_b = label_lengths[b] (a host-side sum over lengths the data
-     *  loader has anyway).  The kept numerators are indexed by compact tile slots, but only the device knows how many tiles
+     *  loader has anyway); with the windows of the _windowed entries, at most N tiles are valid under their rule.  The kept numerators are indexed by compact tile slots, but only the device knows how many tiles
      *  are valid (the library never synchronises with the host), so by default the workspace is sized for every tile of
      *  the padded (maxT, maxU) lattice and a batch whose padded numerators exceed 16 GiB is processed in utterance chunks,
      *  which rules keep_activations out.  With a bound the workspace holds N row blocks and the batch is one chunk.  If
@@ -241,6 +241,59 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
                                                    const int* label_lengths, const int* input_lengths,
                                                    const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                                    float* db, void* workspace, float fastemit_lambda);
+
+/** Alignment-restricted RNN-T (Mahadeokar et al., "Alignment Restricted Streaming Recurrent Neural Network Transducer",
+ *  SLT 2021): the loss sums only over the paths that stay inside per-label time windows.  Per utterance b and lattice
+ *  column u in [0, U_b), U_b = label_lengths[b] + 1, the caller gives an inclusive frame window [t_lo[b,u], t_hi[b,u]]:
+ *  two int32 DEVICE arrays (B, maxU), row stride maxU, entries at u >= U_b ignored.  Cell (t,u) is ALLOWED iff
+ *  t_lo[b,u] <= t <= t_hi[b,u] and t < T_b.  Any int32 is accepted and nothing is clamped: t_lo > t_hi, or a window outside
+ *  [0, T_b), is an empty column.  BOTH ARCS LEAVING A CELL THAT IS NOT ALLOWED HAVE LOG-PROBABILITY -inf, as does the
+ *  terminating blank at (T_b-1, U_b-1) if that cell is not allowed; equivalently
+ *    costs[b] = -log sum P(path) over the paths that visit allowed cells only.
+ *  Everything else (softmax inside, blank, labels, grad_costs, FastEmit's (1 + lambda) on label arcs, padded cells written
+ *  0) is as in the entries without windows.  Consequences:
+ *    - the gradients of the logits of a cell that is not allowed are exactly 0;
+ *    - windows that cover the lattice (t_lo <= 0, t_hi >= T_b - 1) give costs and gradients bit-identical to the entries
+ *      without windows, which are these entries with t_lo == t_hi == NULL;
+ *    - windows that admit no path give costs[b] = +inf and exactly-zero gradients for that utterance, no NaN, and leave
+ *      the other utterances of the batch untouched.
+ *  The forward AND the backward entry take the windows (they change the costs), and must be given the same ones.
+ *  Exactly one of t_lo / t_hi NULL -> RNNT_STATUS_INVALID_VALUE before any device work.
+ *  On the tensor-core joint path a 16 x 8 lattice tile (b, t0, u0) is VALID iff it intersects the T_b x U_b lattice and
+ *  some column u in [u0, min(u0 + 8, U_b)) has [t_lo, t_hi] meet [t0, t0 + 16); tiles that are not valid are never
+ *  computed, in the forward or in either backward GEMM, and take no room among the kept numerators.
+ *  rnntb200JointDesc.valid_tile_bound keeps its meaning under this rule ("at most N tiles are valid"; a broken promise
+ *  gives NaN costs and no out-of-bounds write).  The loss op and the fp32 joint path skip the logits of cells that are not
+ *  allowed in their softmax and gradient passes (the fp32 joint path still projects them).
+ *  rnntb200_loss_device_windowed: rnntb200_loss_device_fastemit with windows. */
+rnntStatus_t rnntb200_loss_device_windowed(const float* activations, float* gradients, const int* flat_labels,
+                                           const int* label_lengths, const int* input_lengths, const float* grad_scale,
+                                           const int* t_lo, const int* t_hi, int alphabet_size, int minibatch,
+                                           float* costs_device, void* workspace, rnntOptions options,
+                                           float fastemit_lambda);
+
+/** rnntb200_loss16_forward / rnntb200_loss16_backward_fastemit with windows (see rnntb200_loss_device_windowed). */
+rnntStatus_t rnntb200_loss16_forward_windowed(const void* activations, int logit_type, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                              const int* t_hi, int alphabet_size, int minibatch, float* costs_device,
+                                              void* workspace, rnntOptions options);
+rnntStatus_t rnntb200_loss16_backward_windowed(const void* activations, int logit_type, const int* flat_labels,
+                                               const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                               const int* t_hi, const float* grad_costs, int alphabet_size, int minibatch,
+                                               void* gradients, const void* workspace, rnntOptions options,
+                                               float fastemit_lambda);
+
+/** rnntb200_joint_loss_forward / rnntb200_joint_loss_backward_fastemit with windows (see rnntb200_loss_device_windowed),
+ *  both precisions; the descriptor keeps its layout.  The windowed backward is as deterministic as the plain one. */
+rnntStatus_t rnntb200_joint_loss_forward_windowed(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                  const float* W, const float* bias, const int* labels,
+                                                  const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                                  const int* t_hi, float* costs, void* workspace);
+rnntStatus_t rnntb200_joint_loss_backward_windowed(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                   const float* W, const float* bias, const int* labels,
+                                                   const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                                   const int* t_hi, const float* grad_costs, float* d_enc, float* d_pred,
+                                                   float* dW, float* db, void* workspace, float fastemit_lambda);
 
 /** Forced alignment: the single most likely path through the lattice the loss sums over (Viterbi), per utterance b
  *  with T = input_lengths[b], U = label_lengths[b] + 1 and the log-probs of the loss, lpb(t,u) at blank and lpl(t,u)

@@ -32,6 +32,8 @@ EXPORTS = ("get_warprnnt_version", "rnntGetStatusString", "get_workspace_size", 
            "rnntb200_loss_device_fastemit", "rnntb200_loss16_backward_fastemit",
            "rnntb200_joint_workspace_size",
            "rnntb200_joint_loss_forward", "rnntb200_joint_loss_backward", "rnntb200_joint_loss_backward_fastemit",
+           "rnntb200_loss_device_windowed", "rnntb200_loss16_forward_windowed", "rnntb200_loss16_backward_windowed",
+           "rnntb200_joint_loss_forward_windowed", "rnntb200_joint_loss_backward_windowed",
            "rnntb200_align_device", "rnntb200_align16", "rnntb200_joint_align",
            "rnntb200_joint_logits", "rnntb200_joint_step",
            "rnntb200_dense1_forward", "rnntb200_dense1_backward",
@@ -75,6 +77,11 @@ def load(build_if_missing=True):
     L.rnntb200_joint_loss_forward.argtypes = [C.POINTER(JointDesc)] + [vp] * 9
     L.rnntb200_joint_loss_backward.argtypes = [C.POINTER(JointDesc)] + [vp] * 13
     L.rnntb200_joint_loss_backward_fastemit.argtypes = L.rnntb200_joint_loss_backward.argtypes + [C.c_float]
+    L.rnntb200_loss_device_windowed.argtypes = [vp] * 8 + [ci, ci, vp, vp, RnntOptions, C.c_float]
+    L.rnntb200_loss16_forward_windowed.argtypes = [vp, ci] + [vp] * 5 + [ci, ci, vp, vp, RnntOptions]
+    L.rnntb200_loss16_backward_windowed.argtypes = [vp, ci] + [vp] * 6 + [ci, ci, vp, vp, RnntOptions, C.c_float]
+    L.rnntb200_joint_loss_forward_windowed.argtypes = [C.POINTER(JointDesc)] + [vp] * 11
+    L.rnntb200_joint_loss_backward_windowed.argtypes = [C.POINTER(JointDesc)] + [vp] * 15 + [C.c_float]
     L.rnntb200_align_device.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, RnntOptions]
     L.rnntb200_align16.argtypes = [vp, ci, vp, vp, vp, ci, ci, vp, vp, vp, vp, RnntOptions]
     L.rnntb200_joint_align.argtypes = [C.POINTER(JointDesc)] + [vp] * 11

@@ -55,8 +55,9 @@ struct BwdParams {
 // ---------------------------------------------------------------------------------------------------------------
 // dZ kernel
 // ---------------------------------------------------------------------------------------------------------------
-// Work order (identical in both roles): runs = (utterance, t-block) assigned round-robin to CTAs; inside a run the valid
-// tiles along u; inside a tile ceil(H / 128) passes of 128 columns (the last pass of an H % 128 == 64 model reads W rows
+// Work order (identical in both roles): runs = (utterance, t-block) assigned round-robin to CTAs; inside a run the tiles
+// along u that have a slot (with windows most tiles of a run have none, at its start as well as its end: both roles skip
+// them in lock-step, and a run without any stores its d_enc rows as zeros); inside a tile ceil(H / 128) passes of 128 columns (the last pass of an H % 128 == 64 model reads W rows
 // past H as TMA zero fill and stores nothing for them).  A stage = the tile's E' block [128 rows x 64 v] + the pass's W
 // rows [128 h x 64 v].  Besides the ring, one input slot holds the pass's enc rows [16 t x 128 h] and pred rows
 // [8 u x 128 h] (fp32 boxes, rows past the arrays read as 0) for the epilogue: the TMA lane loads it halfway through the
@@ -102,7 +103,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                 const int nub = (Un + BW_UU - 1) / BW_UU;
                 for (int ub = 0; ub < nub; ++ub) {
                     const int tile = (bl * p.nTb + tb) * p.nUb + ub;
-                    const int sl = max(p.slot ? p.slot[tile] : tile, 0);   // a slot-less tile (broken bound) has rs = 0 everywhere
+                    const int sl = p.slot ? p.slot[tile] : tile;
+                    if (sl < 0) continue;                                    // no slot: outside the windows (or a broken bound)
                     for (int pass = 0; pass < NPASS; ++pass)
                         for (int kb = 0; kb < KBV; ++kb) {
                             if (kb == KBV / 2) {
@@ -137,11 +139,12 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
         const int nub = (Un + BW_UU - 1) / BW_UU;
         for (int ub = 0; ub < nub; ++ub) {
             const int tile = (bl * p.nTb + tb) * p.nUb + ub;
-            const int tslot = p.slot ? p.slot[tile] : tile;               // < 0 only after a broken valid_tile_bound promise
+            const int tslot = p.slot ? p.slot[tile] : tile;
+            if (tslot < 0) continue;            // as the TMA role: its d_pred partial plane is not written, and not summed
             float rs[2];
 #pragma unroll
-            for (int ri = 0; ri < 2; ++ri)      // 0 outside the lattice
-                rs[ri] = tslot >= 0 ? __ldg(p.rowscale + (size_t)tslot * 128 + Ra + 8 * ri) : 0.f;
+            for (int ri = 0; ri < 2; ++ri)      // 0 outside the lattice and the windows
+                rs[ri] = __ldg(p.rowscale + (size_t)tslot * 128 + Ra + 8 * ri);
             for (int pass = 0; pass < NPASS; ++pass) {
                 const int n0 = pass * DZ_NC;
                 float acc[64];
@@ -237,8 +240,10 @@ inline DzGeom dz_geometry(int H) {
     return g;
 }
 
-// d_pred[b,u,:] = sum over the t-blocks that intersect the utterance of its partial planes (0 for u >= U_b)
-__global__ void __launch_bounds__(256) sum_pred_planes_kernel(const float4* __restrict__ ppred, const int* __restrict__ xlen,
+// d_pred[b,u,:] = sum over the t-blocks that intersect the utterance of its partial planes (0 for u >= U_b), in t-block
+// order.  bwd_dz_kernel writes a plane's rows only for tiles that have a slot, so the others are left out of the sum.
+__global__ void __launch_bounds__(256) sum_pred_planes_kernel(const float4* __restrict__ ppred, const int* __restrict__ slot,
+                                                              int nTb, int nUb, const int* __restrict__ xlen,
                                                               const int* __restrict__ ylen, int b0, int nb, int maxU, int H4,
                                                               float4* __restrict__ d_pred) {
     const size_t n4 = (size_t)nb * maxU * H4;
@@ -249,6 +254,7 @@ __global__ void __launch_bounds__(256) sum_pred_planes_kernel(const float4* __re
             const int ntb = (xlen[b] + BW_TT - 1) / BW_TT;
 #pragma unroll 4
             for (int k = 0; k < ntb; ++k) {
+                if (slot[(bl * nTb + k) * nUb + u / BW_UU] < 0) continue;
                 const float4 v = ppred[(size_t)k * n4 + i];
                 acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
             }

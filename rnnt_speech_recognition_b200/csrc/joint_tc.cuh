@@ -67,7 +67,21 @@ struct JointTcParams {
     // per lattice cell, gm the row's reference ref (log2 domain).
     __nv_bfloat16* dl;
     float* gm;
+    Windows win;                // alignment-restricted loss: per-column frame windows (lo == NULL: none)
 };
+// THE validity rule of a TT x UU tile at (b, t0, u0), shared by tile_compact_kernel (slots) and decode_tile (forward):
+// the tile intersects the utterance's T_b x U_b lattice and, with windows, some column u in [u0, min(u0 + UU, U_b)) has
+// [lo, hi] meet [t0, t0 + TT).  Full windows (lo <= 0, hi >= T_b - 1) therefore rank the tiles exactly as no windows do.
+__device__ __forceinline__ bool tile_valid(int b, int t0, int u0, int Tn, int Un, int TT, int UU, int maxU, const Windows& w) {
+    if (!(t0 < Tn && u0 < Un)) return false;
+    if (!w.lo) return true;
+    const int u1 = min(u0 + UU, Un);
+    for (int u = u0; u < u1; ++u) {
+        const int lo = w.lo[(long long)b * maxU + u], hi = w.hi[(long long)b * maxU + u];
+        if (lo <= hi && lo < t0 + TT && hi >= t0) return true;
+    }
+    return false;
+}
 struct TileInfo { int b, t0, u0, Tn, Un; bool valid; };
 __device__ __forceinline__ TileInfo decode_tile(const JointTcParams& p, int tile) {
     TileInfo ti;
@@ -78,7 +92,7 @@ __device__ __forceinline__ TileInfo decode_tile(const JointTcParams& p, int tile
     ti.u0 = (rem % p.nUb) * p.UU;
     ti.Tn = p.xlen[ti.b];
     ti.Un = p.ylen[ti.b] + 1;
-    ti.valid = ti.t0 < ti.Tn && ti.u0 < ti.Un;
+    ti.valid = tile_valid(ti.b, ti.t0, ti.u0, ti.Tn, ti.Un, p.TT, p.UU, p.maxU, p.win);
     return ti;
 }
 
@@ -101,14 +115,15 @@ __global__ void __launch_bounds__(256) convert_w_kernel(const float* __restrict_
     }
 }
 
-// slot[tile] = rank of the tile among the VALID tiles of this launch (-1 if it lies in the padding); *count = #valid.
+// slot[tile] = rank of the tile among the VALID tiles (tile_valid) of this launch (-1 for the others); *count = #valid.
 // One block; a serial-over-chunks block scan is plenty for the <= ~1e5 tiles of a launch.
 __global__ void __launch_bounds__(1024) tile_compact_kernel(const int* __restrict__ xlen, const int* __restrict__ ylen,
                                                             int b0, int ntiles, int nTb, int nUb, int TT, int UU,
                                                             int* __restrict__ slot, int* __restrict__ count,
                                                             int* __restrict__ tile_of_slot = nullptr,
                                                             int4* __restrict__ slot_meta = nullptr, int maxT = 0, int maxU = 0,
-                                                            int max_slots = 0x7fffffff) {
+                                                            int max_slots = 0x7fffffff,
+                                                            const Windows win = Windows{nullptr, nullptr}) {
     __shared__ int warp_sums[32];
     __shared__ int base;
     if (threadIdx.x == 0) base = 0;
@@ -121,7 +136,7 @@ __global__ void __launch_bounds__(1024) tile_compact_kernel(const int* __restric
         if (tile < ntiles) {
             const int bl = tile / per_utt, rem = tile - bl * per_utt, b = b0 + bl;
             const int tt = (rem / nUb) * TT, uu = (rem % nUb) * UU;
-            v = (tt < xlen[b] && uu < ylen[b] + 1) ? 1 : 0;
+            v = tile_valid(b, tt, uu, xlen[b], ylen[b] + 1, TT, UU, maxU, win) ? 1 : 0;
             // what the kernels that walk the compact slots need of a tile, so that none of them divides: first enc / pred row
             // (in rows of H floats) and how many of the tile's TT / UU rows exist in the padded arrays
             meta = make_int4(b * maxT + tt, b * maxU + uu, min(TT, maxT - tt), min(UU, maxU - uu));
@@ -332,7 +347,7 @@ template <bool KEEP>
 inline rnntStatus_t tc_run_forward(const rnntb200JointDesc& d, const TcGeom& g, const TcScratch& sc, const float* enc,
                                    const float* pred, const float* bias, const int* labels, const int* ylen,
                                    const int* xlen, float* lse, float* lpb, float* lpl, int b0, int nb, cudaStream_t s,
-                                   unsigned* launches) {
+                                   unsigned* launches, const Windows& win) {
     const FwdGeom fg = fwd_geometry(d.H, d.V);
     JointTcParams p{};
     p.enc = enc; p.pred = pred; p.bias = bias; p.labels = labels; p.xlen = xlen; p.ylen = ylen;
@@ -342,10 +357,11 @@ inline rnntStatus_t tc_run_forward(const rnntb200JointDesc& d, const TcGeom& g, 
     p.b0 = b0; p.nb = nb;
     p.lse = lse; p.lpb = lpb; p.lpl = lpl;
     p.stages = fg.stages;
+    p.win = win;
     if (KEEP) {
         const int ntiles = nb * g.nTb * g.nUb;
         tile_compact_kernel<<<1, 1024, 0, s>>>(xlen, ylen, b0, ntiles, g.nTb, g.nUb, g.TT, g.UU, sc.slot, sc.count, sc.tile_of_slot, sc.slot_meta,
-                                             d.maxT, d.maxU, (int)(sc.rows_chunk / 128));
+                                             d.maxT, d.maxU, (int)(sc.rows_chunk / 128), win);
         *launches += 1;
         p.slot = sc.slot; p.dl = sc.dl; p.gm = sc.gm;
     }
@@ -361,15 +377,15 @@ inline rnntStatus_t tc_run_forward(const rnntb200JointDesc& d, const TcGeom& g, 
 inline rnntStatus_t tc_forward(const rnntb200JointDesc& d, void* scratch, const float* enc, const float* pred,
                                const float* W, const float* bias, const int* labels, const int* ylen,
                                const int* xlen, float* lse, float* lpb, float* lpl, cudaStream_t s,
-                               unsigned* launches) {
+                               unsigned* launches, const Windows& win) {
     if (!tc_supported(d)) return tc_unsupported(d);
     const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
     TcScratch sc = tc_scratch_layout(d, scratch);
     convert_w_kernel<<<dim3((d.V + 31) / 32, (d.H + 31) / 32), 256, 0, s>>>(W, sc.Wt, sc.Wb, d.H, d.V);
     *launches += 1;
     if (tc_keep(d, sc))
-        return tc_run_forward<true>(d, g, sc, enc, pred, bias, labels, ylen, xlen, lse, lpb, lpl, 0, d.B, s, launches);
-    return tc_run_forward<false>(d, g, sc, enc, pred, bias, labels, ylen, xlen, lse, lpb, lpl, 0, d.B, s, launches);
+        return tc_run_forward<true>(d, g, sc, enc, pred, bias, labels, ylen, xlen, lse, lpb, lpl, 0, d.B, s, launches, win);
+    return tc_run_forward<false>(d, g, sc, enc, pred, bias, labels, ylen, xlen, lse, lpb, lpl, 0, d.B, s, launches, win);
 }
 
 // The valid_tile_bound promise of a call that keeps nothing (alignment): when a bound is given and the batch is one
@@ -392,12 +408,13 @@ struct LossPlanes { const float *lse, *lpb, *lpl, *alphas, *betas, *llf; };   //
 // Backward (SURVEY 8 a19) with the library's own wgmma kernels (joint_bwd.cuh).  Per utterance chunk: (a keeping forward
 // of the chunk unless the forward call already kept the whole batch) -> row_scale_kernel -> bwd_dz_kernel -> d_pred plane
 // sum -> bwd_dw_kernel; after the last chunk the split-K planes of dW / db are summed.  Stream-ordered, no host
-// synchronisation, no library calls.  FastEmit lives entirely in row_scale_kernel (every chunk, keep or recompute): the
+// synchronisation, no library calls.  Windows reach the backward through the slots (tiles outside them have none),
+// row_scale_kernel (rows outside them get rs = 0) and nothing else.  FastEmit lives entirely in row_scale_kernel (every chunk, keep or recompute): the
 // GEMM kernels consume E' as they always do.
 inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const float* enc, const float* pred,
                                 const float* bias, const int* labels, const int* ylen, const int* xlen,
                                 const LossPlanes& lp, const float* grad_costs, float* d_enc, float* d_pred, float* dW,
-                                float* db, cudaStream_t s, unsigned* launches, float fastemit_lambda) {
+                                float* db, cudaStream_t s, unsigned* launches, float fastemit_lambda, const Windows& win) {
     if (!tc_supported(d)) return tc_unsupported(d);
     const TcGeom g = tc_geometry(d.maxT, d.maxU, d.H, d.V);
     const DzGeom zg = dz_geometry(d.H);
@@ -420,7 +437,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
     for (int b0 = 0; b0 < d.B; b0 += sc.bchunk) {
         const int nb = (d.B - b0 < sc.bchunk) ? d.B - b0 : sc.bchunk;
         if (!kept) {
-            rnntStatus_t st = tc_run_forward<true>(d, g, sc, enc, pred, bias, labels, ylen, xlen, nullptr, nullptr, nullptr, b0, nb, s, launches);
+            rnntStatus_t st = tc_run_forward<true>(d, g, sc, enc, pred, bias, labels, ylen, xlen, nullptr, nullptr, nullptr, b0, nb, s, launches, win);
             if (st) return st;
         }
         {   // per-row scales of this chunk (row order of the kept arrays) + the two special columns of every row
@@ -428,7 +445,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
             row_scale_kernel<<<(unsigned)(((size_t)nb * g.nTb * g.nUb * 128 + 255) / 256), 256, 0, s>>>(
                 sc.tile_of_slot, sc.count, b0, g.nTb, g.nUb, xlen, ylen, labels, d.blank_label, d.maxT, d.maxU,
                 (long long)(d.maxT + d.maxU - 1) * d.maxU, lp.lse, lp.lpb, lp.lpl, lp.alphas, lp.betas, lp.llf, grad_costs, sc.gm,
-                d.V, reinterpret_cast<unsigned short*>(sc.dl), sc.rowscale, fastemit_lambda);
+                d.V, reinterpret_cast<unsigned short*>(sc.dl), sc.rowscale, fastemit_lambda, win);
             *launches += 1;
         }
         BwdParams p{};
@@ -438,7 +455,8 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         p.slot = sc.slot; p.slot_meta = sc.slot_meta; p.count = sc.count; p.rowscale = sc.rowscale;
         p.dz_stages = zg.stages; p.d_enc = d_enc; p.ppred = sc.ppl;
         p.nVT = wg.nVT; p.nHB = wg.nHB; p.S = wg.S; p.dWp = sc.dWp; p.dbp = sc.dbp;
-        // rows of d_enc whose t-block lies outside the utterance are never visited by the dZ kernel
+        // rows of d_enc whose t-block lies outside the utterance are never visited by the dZ kernel (a t-block inside it
+        // without a valid tile is: its rows are stored as the zeros they are)
         if (cudaMemsetAsync(d_enc + (size_t)b0 * d.maxT * d.H, 0, sizeof(float) * (size_t)nb * d.maxT * d.H, s) != cudaSuccess)
             return RNNT_STATUS_MEMOPS_FAILED;
         {
@@ -450,7 +468,8 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
             const size_t n4 = (size_t)nb * d.maxU * d.H / 4;
             ScopedTimer tmr("sum_pred_planes_kernel", s);
             sum_pred_planes_kernel<<<(unsigned)((n4 + 255) / 256 < 4096 ? (n4 + 255) / 256 : 4096), 256, 0, s>>>(
-                reinterpret_cast<const float4*>(sc.ppl), xlen, ylen, b0, nb, d.maxU, d.H / 4, reinterpret_cast<float4*>(d_pred));
+                reinterpret_cast<const float4*>(sc.ppl), sc.slot, g.nTb, g.nUb, xlen, ylen, b0, nb, d.maxU, d.H / 4,
+                reinterpret_cast<float4*>(d_pred));
         }
         {
             ScopedTimer tmr("bwd_dw_kernel", s);

@@ -8,6 +8,8 @@
 //                       (replaces gpu_rnnt_kernel.h:11-47, 79-113; arithmetic of cpu_rnnt.h:175-253)
 //   rnnt_grad_kernel    gradient w.r.t. logits (gpu_rnnt_kernel.h:143-179), padded cells zeroed
 //                       in the same pass (replaces the cudaMemsetAsync of gpu_rnnt.h:109)
+//   alpha_beta_windowed_kernel   the same wavefronts under the alignment-restricted loss's per-column frame windows
+//                       (struct Windows); lse_gather, rnnt_grad and row_scale take the windows too
 //   row_scale_kernel    per-row scales of the tensor-core backward GEMMs + the patch of the two special columns
 //   zgen/sgemm/...      fp32 building blocks of the exact (RNNTB200_FP32_EXACT) joint path, and colsum (also dense1's db1)
 // lse_gather and rnnt_grad also take fp16 / bf16 logits (and write gradients of that type) over fp32 arithmetic; their
@@ -141,6 +143,19 @@ __device__ __forceinline__ T fastemit_rho(T lp_label, T beta_next_u, T beta) {
     return r < T(1) ? r : T(1);
 }
 
+// Alignment-restricted loss: per utterance b and lattice column u an inclusive frame window [lo[b*maxU+u], hi[b*maxU+u]]
+// (int32, row stride maxU, entries at u >= U_b ignored).  Cell (t,u) is ALLOWED iff lo <= t <= hi (and t < T_b); both arcs
+// leaving a cell that is not allowed have log-probability -inf.  Nothing is clamped: an empty or out-of-range window is an
+// empty column.  lo == NULL: no restriction (every cell of the lattice is allowed).
+struct Windows {
+    const int* lo; const int* hi;
+    __device__ __forceinline__ bool allows(int b, int t, int u, int maxU) const {
+        if (!lo) return true;
+        const long long k = (long long)b * maxU + u;
+        return t >= lo[k] && t <= hi[k];
+    }
+};
+
 struct CellIdx { int b, t, u; };
 __device__ __forceinline__ CellIdx decode_cell(long long cell, int maxT, int maxU) {
     CellIdx c;
@@ -161,6 +176,8 @@ struct RowCell {
     long long cell;
     int b, t, u, Tn, Un;
     __device__ bool padded() const { return t >= Tn || u >= Un; }
+    // padded, or outside the column's window: the cell is never read downstream and its gradient row is 0
+    __device__ bool skipped(const Windows& w, int maxU) const { return padded() || !w.allows(b, t, u, maxU); }
     __device__ long long sk(int maxU, long long SK) const { return sk_index(b, t, u, maxU, SK); }
     // labels[b][u], -1 on the last column (no label arc)
     __device__ int label(const int* labels, int maxU) const { return u < Un - 1 ? labels[(long long)b * (maxU - 1) + u] : -1; }
@@ -169,6 +186,11 @@ __device__ __forceinline__ RowCell row_cell(long long cell, int maxT, int maxU, 
     const CellIdx c = decode_cell(cell, maxT, maxU);
     return {cell, c.b, c.t, c.u, xlen[c.b], ylen[c.b] + 1};
 }
+
+// Windows that admit no path leave ll = -inf: the utterance's cost is +inf and its gradients are exactly 0 (alpha + beta
+// - ll is never formed for it).  Without windows ll is used as it comes.
+template <typename T>
+__device__ __forceinline__ bool win_infeasible(const Windows& w, T ll) { return w.lo && ll == neg_inf<T>(); }
 
 // lane 0 of lse_gather: the row's log-softmax denominator (natural order) and its blank / label log-probs (skewed)
 template <typename T, typename X>
@@ -217,12 +239,12 @@ __global__ void __launch_bounds__(256) lse_gather_kernel(const X* __restrict__ l
                                                          const int* __restrict__ ylen,
                                                          const int* __restrict__ labels, int maxT, int maxU,
                                                          long long SK, int blank, T* __restrict__ lse,
-                                                         T* __restrict__ lpb, T* __restrict__ lpl) {
+                                                         T* __restrict__ lpb, T* __restrict__ lpl, const Windows win) {
     const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
     const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
-    if (c.padded()) return;
+    if (c.skipped(win, maxU)) return;
     const X* x = logits + row * (long long)V;
     T m = neg_inf<T>();
     for (int v = lane; v < V; v += 32) { T xv = widen(x[v]); m = xv > m ? xv : m; }
@@ -242,13 +264,14 @@ __global__ void __launch_bounds__(256) lse_gather_vec_kernel(const X* __restrict
                                                              const int* __restrict__ ylen,
                                                              const int* __restrict__ labels, int maxT, int maxU,
                                                              long long SK, int blank, float* __restrict__ lse,
-                                                             float* __restrict__ lpb, float* __restrict__ lpl) {
+                                                             float* __restrict__ lpb, float* __restrict__ lpl,
+                                                             const Windows win) {
     using P = Vec16<X>;
     const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
     const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
-    if (c.padded()) return;
+    if (c.skipped(win, maxU)) return;
     const X* x = logits + row * (long long)V;
     const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
     const int nv = V >> P::LOG2N;
@@ -298,7 +321,8 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
                                                             const float* __restrict__ alphas,
                                                             const float* __restrict__ betas,
                                                             const float* __restrict__ llf,
-                                                            const float* __restrict__ gscale, float fastemit_lambda) {
+                                                            const float* __restrict__ gscale, float fastemit_lambda,
+                                                            const Windows win) {
     using P = Vec16<X>;
     const long long row = warp_row();
     const int lane = threadIdx.x & 31;
@@ -308,7 +332,7 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
     const typename P::Raw* xv = reinterpret_cast<const typename P::Raw*>(x);
     typename P::Raw* gv = reinterpret_cast<typename P::Raw*>(out + row * (long long)V);
     const int nv = V >> P::LOG2N;
-    if (c.padded()) {
+    if (c.skipped(win, maxU) || win_infeasible(win, llf[c.b])) {
         const float z[P::N] = {};
         for (int k = lane; k < nv; k += 32) gv[k] = P::narrow(z);
         return;
@@ -354,11 +378,15 @@ __global__ void __launch_bounds__(256) rnnt_grad_vec_kernel(const X* logits, X* 
 // ballot word, bit (u & 31) set when the label arc is STRICTLY greater (a tie goes to the blank arc):
 //   dec[b*SKW + n*decw + (u >> 5)],  SKW = (maxT+maxU-1)*decw,  decw = ceil(maxU / 32).
 // ---------------------------------------------------------------------------------------------
-template <typename T, int PF, bool BETA, bool VIT = false>
+// WIN (alignment-restricted loss, struct Windows): thread u holds its column's window in two registers and a cell outside
+// it FETCHES both log-probs as -inf, which is off the dependent chain; the recurrences themselves are unchanged.  The
+// planes of cells outside the windows are never read, so nothing has to fill them.
+template <typename T, int PF, bool BETA, bool VIT = false, bool WIN = false>
 __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const T* __restrict__ lpl, T* __restrict__ out,
                                                 T* __restrict__ ll, const int* __restrict__ xlen,
                                                 const int* __restrict__ ylen, int maxU, long long SK,
-                                                unsigned* __restrict__ dec = nullptr, int decw = 0) {
+                                                unsigned* __restrict__ dec = nullptr, int decw = 0,
+                                                const Windows win = Windows{nullptr, nullptr}) {
     static_assert(!(VIT && BETA), "the Viterbi walk runs forward");
     const int b = blockIdx.x;
     const int u = threadIdx.x, lane = u & 31, warp = u >> 5;
@@ -397,14 +425,23 @@ __device__ __forceinline__ void alpha_beta_body(const T* __restrict__ lpb, const
     // VIT: this warp's decision word of diagonal 0, one row of decw words per diagonal
     unsigned* pdec = VIT ? dec + (long long)b * (long long)(SK / maxU) * decw + warp : nullptr;
     T cb[PF], cl[PF], nb[PF], nl[PF];
+    int wlo = 0, whi = -1;                            // WIN: this column's window
+    if (WIN && col_ok) { wlo = win.lo[(long long)b * maxU + u]; whi = win.hi[(long long)b * maxU + u]; }
     auto fetch = [&](int i0, T* vb, T* vl) {
 #pragma unroll
         for (int j = 0; j < PF; ++j) {
             const int i = i0 + j;
             const bool ok = col_ok && i >= 0 && i < nsteps;
             const long long off = base + (long long)(ok ? (BETA ? nsteps - 1 - i : i) : 0) * maxU;
-            vb[j] = ok ? lpb[off] : T(0);
-            vl[j] = ok ? lpl[off] : T(0);
+            if constexpr (WIN) {
+                const int t = (BETA ? nsteps - 1 - i : i) - u;
+                const bool in = ok && t >= wlo && t <= whi;
+                vb[j] = in ? lpb[off] : (ok ? NEG : T(0));
+                vl[j] = in ? lpl[off] : (ok ? NEG : T(0));
+            } else {
+                vb[j] = ok ? lpb[off] : T(0);
+                vl[j] = ok ? lpl[off] : T(0);
+            }
         }
     };
     fetch(-lag, nb, nl);
@@ -464,6 +501,18 @@ __global__ void __launch_bounds__(1024) alpha_beta_kernel(const T* __restrict__ 
                                                           const int* __restrict__ ylen, int maxU, long long SK) {
     if (blockIdx.y == 1) alpha_beta_body<T, PF, true>(lpb, lpl, betas, llb, xlen, ylen, maxU, SK);
     else alpha_beta_body<T, PF, false>(lpb, lpl, alphas, llf, xlen, ylen, maxU, SK);
+}
+
+// alpha_beta_kernel of the alignment-restricted loss (fp32): the same walk with the windows applied where the log-probs are
+// fetched.  A kernel of its own, so that the unrestricted kernels keep their code.
+template <int PF>
+__global__ void __launch_bounds__(1024) alpha_beta_windowed_kernel(const float* __restrict__ lpb, const float* __restrict__ lpl,
+                                                                   float* __restrict__ alphas, float* __restrict__ betas,
+                                                                   float* __restrict__ llf, float* __restrict__ llb,
+                                                                   const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                                                   int maxU, long long SK, const Windows win) {
+    if (blockIdx.y == 1) alpha_beta_body<float, PF, true, false, true>(lpb, lpl, betas, llb, xlen, ylen, maxU, SK, nullptr, 0, win);
+    else alpha_beta_body<float, PF, false, false, true>(lpb, lpl, alphas, llf, xlen, ylen, maxU, SK, nullptr, 0, win);
 }
 
 // Forced alignment, step 1: the Viterbi wavefront (alpha_beta_body<VIT>), one CTA per utterance.  Writes the decision
@@ -549,14 +598,14 @@ __global__ void __launch_bounds__(256) rnnt_grad_kernel(const X* logits, X* out,
                                                         long long SK, int blank, const T* __restrict__ lse,
                                                         const T* __restrict__ alphas, const T* __restrict__ betas,
                                                         const T* __restrict__ llf, const T* __restrict__ gscale,
-                                                        float fastemit_lambda) {
+                                                        float fastemit_lambda, const Windows win) {
     const long long row = warp_row();
     const int lane = threadIdx.x & 31;
     if (row >= nrows) return;
     const RowCell c = row_cell(row0 + row, maxT, maxU, xlen, ylen);
     const X* x = logits + row * (long long)V;
     X* g = out + row * (long long)V;
-    if (c.padded()) {
+    if (c.skipped(win, maxU) || win_infeasible(win, llf[c.b])) {
         for (int v = lane; v < V; v += 32) g[v] = narrow<X>(T(0));
         return;
     }
@@ -596,7 +645,7 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
                                                         const float* __restrict__ betas, const float* __restrict__ llf,
                                                         const float* __restrict__ gscale, const float* __restrict__ rowref, int V,
                                                         unsigned short* __restrict__ E, float* __restrict__ rowscale,
-                                                        float fastemit_lambda) {
+                                                        float fastemit_lambda, const Windows win) {
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int sl = (int)(row >> 7), r = (int)(row & 127);
     if (sl >= *count) return;
@@ -605,7 +654,9 @@ __global__ void __launch_bounds__(256) row_scale_kernel(const int* __restrict__ 
     const int t = (rem / nUb) * 16 + (r >> 3), u = (rem % nUb) * 8 + (r & 7);
     const int Tn = xlen[b], Un = ylen[b] + 1;
     float rs = 0.f;
-    if (t < Tn && u < Un) {
+    // (rows outside their column's window, and every row of an utterance whose windows admit no path, keep rs = 0 and
+    //  their E untouched: nothing of theirs reaches a gradient)
+    if (t < Tn && u < Un && win.allows(b, t, u, maxU) && !win_infeasible(win, llf[b])) {
         const long long k = sk_index(b, t, u, maxU, SK);
         const float a = alphas[k], bt = betas[k], ll = llf[b], g = gscale ? gscale[b] : 1.f;
         const float occ = a + bt - ll;                                   // log occupancy of the cell

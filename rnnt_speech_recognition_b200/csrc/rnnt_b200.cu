@@ -60,6 +60,11 @@ __global__ void finish_costs_kernel(const float* __restrict__ llf, const float* 
     if (diff > 0.1f) printf("WARNING: Forward backward likelihood mismatch %f (utterance %d)\n", diff, i);
 }
 
+// The windows of the alignment-restricted entries (rb::Windows); the entries without them pass none.  Both pointers or
+// neither: exactly one NULL is an argument error.
+constexpr rb::Windows no_windows{nullptr, nullptr};
+inline bool windows_ok(const int* t_lo, const int* t_hi) { return (t_lo == nullptr) == (t_hi == nullptr); }
+
 inline rnntStatus_t check_launch() { return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED; }
 
 // overflow (nullable): the tensor-core forward's broken valid_tile_bound word, which turns the costs into NaN
@@ -71,12 +76,18 @@ rnntStatus_t launch_finish_costs(const float* llf, const float* llb, float* cost
 
 template <typename T>
 rnntStatus_t launch_alpha_beta(const LossWs<T>& w, const int* xlen, const int* ylen, int B, int maxT, int maxU,
-                               cudaStream_t s) {
+                               cudaStream_t s, const rb::Windows& win = no_windows) {
     const int threads = (maxU + 31) / 32 * 32;
     constexpr int PF = sizeof(T) == 4 ? 8 : 4;
     rb::ScopedTimer tm("alpha_beta_kernel", s);
-    rb::alpha_beta_kernel<T, PF><<<dim3(B, 2), threads, 0, s>>>(w.lpb, w.lpl, w.alphas, w.betas, w.llf, w.llb, xlen,
-                                                                ylen, maxU, skew_plane(maxT, maxU));
+    if constexpr (sizeof(T) == 4) {
+        if (win.lo)
+            rb::alpha_beta_windowed_kernel<PF><<<dim3(B, 2), threads, 0, s>>>(w.lpb, w.lpl, w.alphas, w.betas, w.llf, w.llb,
+                                                                              xlen, ylen, maxU, skew_plane(maxT, maxU), win);
+    }
+    if (sizeof(T) != 4 || !win.lo)
+        rb::alpha_beta_kernel<T, PF><<<dim3(B, 2), threads, 0, s>>>(w.lpb, w.lpl, w.alphas, w.betas, w.llf, w.llb, xlen,
+                                                                    ylen, maxU, skew_plane(maxT, maxU));
     RB_LAUNCHED(1);
     return check_launch();
 }
@@ -118,7 +129,8 @@ bool vec_ok(const X* acts, const X* grads, int V) {
 // X is the logits' element type: T itself, or fp16 / bf16 over a float workspace.
 template <typename T, typename X>
 rnntStatus_t loss_planes(const X* acts, bool vec, const int* labels, const int* ylen, const int* xlen, int V, int B,
-                         int maxT, int maxU, int blank, void* workspace, cudaStream_t s) {
+                         int maxT, int maxU, int blank, void* workspace, cudaStream_t s,
+                         const rb::Windows& win = no_windows) {
     if (maxU > 1024) {
         fprintf(stderr, "rnnt_b200: maxU=%d exceeds the 1024 label positions per utterance limit\n", maxU);
         return RNNT_STATUS_INVALID_VALUE;
@@ -132,19 +144,19 @@ rnntStatus_t loss_planes(const X* acts, bool vec, const int* labels, const int* 
             if (vec) {
                 if (V <= 8 * 32 * (16 / (int)sizeof(X)))      // 8 pieces of 16 bytes per lane held in registers
                     rb::lse_gather_vec_kernel<X, 8><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                                           blank, w.lse, w.lpb, w.lpl);
+                                                                           blank, w.lse, w.lpb, w.lpl, win);
                 else
                     rb::lse_gather_vec_kernel<X, 0><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                                           blank, w.lse, w.lpb, w.lpl);
+                                                                           blank, w.lse, w.lpb, w.lpl, win);
             }
         }
         if (!vec)
             rb::lse_gather_kernel<T, X><<<blocks, 256, 0, s>>>(acts, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
-                                                               w.lse, w.lpb, w.lpl);
+                                                               w.lse, w.lpb, w.lpl, win);
     }
     RB_LAUNCHED(1);
     if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
-    if (launch_alpha_beta(w, xlen, ylen, B, maxT, maxU, s)) return RNNT_STATUS_EXECUTION_FAILED;
+    if (launch_alpha_beta(w, xlen, ylen, B, maxT, maxU, s, win)) return RNNT_STATUS_EXECUTION_FAILED;
     return RNNT_STATUS_SUCCESS;
 }
 
@@ -152,7 +164,7 @@ rnntStatus_t loss_planes(const X* acts, bool vec, const int* labels, const int* 
 template <typename T, typename X>
 rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, const int* ylen, const int* xlen,
                         const T* gscale, int V, int B, int maxT, int maxU, int blank, void* workspace, cudaStream_t s,
-                        float fastemit_lambda) {
+                        float fastemit_lambda, const rb::Windows& win = no_windows) {
     LossWs<T> w(workspace, B, maxT, maxU);
     const long long N = (long long)B * maxT * maxU, SK = skew_plane(maxT, maxU);
     const unsigned blocks = (unsigned)((N * 32 + 255) / 256);
@@ -160,11 +172,11 @@ rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, co
     if constexpr (sizeof(T) == 4) {
         if (vec)
             rb::rnnt_grad_vec_kernel<X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK, blank,
-                                                               w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda);
+                                                               w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda, win);
     }
     if (!vec)
         rb::rnnt_grad_kernel<T, X><<<blocks, 256, 0, s>>>(acts, grads, 0, N, V, xlen, ylen, labels, maxT, maxU, SK,
-                                                          blank, w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda);
+                                                          blank, w.lse, w.alphas, w.betas, w.llf, gscale, fastemit_lambda, win);
     RB_LAUNCHED(1);
     return check_launch();
 }
@@ -172,8 +184,9 @@ rnntStatus_t loss_grads(const X* acts, X* grads, bool vec, const int* labels, co
 // forward of the device-costs entries (fp32 or 16-bit logits over a float workspace): planes, then the costs
 template <typename X>
 rnntStatus_t loss_forward(const X* acts, bool vec, const int* labels, const int* ylen, const int* xlen, int V, int B,
-                          int maxT, int maxU, int blank, float* costs, void* workspace, cudaStream_t s) {
-    rnntStatus_t st = loss_planes<float, X>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s);
+                          int maxT, int maxU, int blank, float* costs, void* workspace, cudaStream_t s,
+                          const rb::Windows& win = no_windows) {
+    rnntStatus_t st = loss_planes<float, X>(acts, vec, labels, ylen, xlen, V, B, maxT, maxU, blank, workspace, s, win);
     if (st) return st;
     const LossWs<float> w(workspace, B, maxT, maxU);
     return launch_finish_costs(w.llf, w.llb, costs, B, nullptr, s);
@@ -322,7 +335,7 @@ void exact_project(const rnntb200JointDesc& d, const float* enc, const float* pr
 
 rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
                            const float* W, const float* bias, const int* labels, const int* ylen, const int* xlen,
-                           cudaStream_t s) {
+                           cudaStream_t s, const rb::Windows& win) {
     const long long N = (long long)d.B * d.maxT * d.maxU, SK = skew_plane(d.maxT, d.maxU);
     float* Z = reinterpret_cast<float*>(ws.scratch);
     float* L = Z + ws.chunk_rows * d.H;
@@ -331,7 +344,7 @@ rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const 
         exact_project(d, enc, pred, W, bias, r0, rows, Z, L, s);
         rb::lse_gather_kernel<float><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
             L, r0, rows, d.V, xlen, ylen, labels, d.maxT, d.maxU, SK, d.blank_label, ws.loss.lse, ws.loss.lpb,
-            ws.loss.lpl);
+            ws.loss.lpl, win);
         RB_LAUNCHED(1);
         if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
     }
@@ -341,7 +354,7 @@ rnntStatus_t exact_forward(const rnntb200JointDesc& d, const JointWs& ws, const 
 rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
                             const float* W, const float* bias, const int* labels, const int* ylen, const int* xlen,
                             const float* grad_costs, float* d_enc, float* d_pred, float* dW, float* db,
-                            cudaStream_t s, float fastemit_lambda) {
+                            cudaStream_t s, float fastemit_lambda, const rb::Windows& win) {
     const long long N = (long long)d.B * d.maxT * d.maxU, SK = skew_plane(d.maxT, d.maxU);
     float* Z = reinterpret_cast<float*>(ws.scratch);
     float* L = Z + ws.chunk_rows * d.H;
@@ -357,7 +370,7 @@ rnntStatus_t exact_backward(const rnntb200JointDesc& d, const JointWs& ws, const
         // dlogits in place (gpu_rnnt_kernel.h:143-179 formula, times the upstream per-utterance gradient)
         rb::rnnt_grad_kernel<float><<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
             L, L, r0, rows, d.V, xlen, ylen, labels, d.maxT, d.maxU, SK, d.blank_label, ws.loss.lse, ws.loss.alphas,
-            ws.loss.betas, ws.loss.llf, grad_costs, fastemit_lambda);
+            ws.loss.betas, ws.loss.llf, grad_costs, fastemit_lambda, win);
         // dZ = dL . W^T      (rows x V) . (V x H):  B(k=v, n=h) = W[h*V + v]
         {
             rb::ScopedTimer tm("sgemm dZ=dL.W^T", s);
@@ -393,16 +406,17 @@ inline rnntStatus_t tc_missing() {
 // its word is fresh; one that keeps nothing counts them only for the alignment (check_bound).
 rnntStatus_t joint_forward(const rnntb200JointDesc& d, const JointWs& ws, const float* enc, const float* pred,
                            const float* W, const float* bias, const int* labels, const int* ylen, const int* xlen,
-                           float* costs, bool check_bound, const int** overflow, cudaStream_t s) {
+                           float* costs, bool check_bound, const int** overflow, cudaStream_t s,
+                           const rb::Windows& win = no_windows) {
     *overflow = nullptr;
     rnntStatus_t st;
     if (d.precision == RNNTB200_FP32_EXACT) {
-        st = exact_forward(d, ws, enc, pred, W, bias, labels, ylen, xlen, s);
+        st = exact_forward(d, ws, enc, pred, W, bias, labels, ylen, xlen, s, win);
     } else {
 #ifndef RNNTB200_NO_TC
         unsigned nl = 0;
         st = rb::tc_forward(d, ws.scratch, enc, pred, W, bias, labels, ylen, xlen, ws.loss.lse, ws.loss.lpb, ws.loss.lpl,
-                            s, &nl);
+                            s, &nl, win);
         if (!st) {
             const rb::TcScratch sc = rb::tc_scratch_layout(d, ws.scratch);
             if (check_bound) *overflow = rb::tc_check_tile_bound(d, ws.scratch, ylen, xlen, s, &nl);
@@ -414,7 +428,7 @@ rnntStatus_t joint_forward(const rnntb200JointDesc& d, const JointWs& ws, const 
 #endif
     }
     if (st) return st;
-    st = launch_alpha_beta(ws.loss, xlen, ylen, d.B, d.maxT, d.maxU, s);
+    st = launch_alpha_beta(ws.loss, xlen, ylen, d.B, d.maxT, d.maxU, s, win);
     if (st) return st;
     return launch_finish_costs(ws.loss.llf, ws.loss.llb, costs, d.B, *overflow, s);
 }
@@ -480,30 +494,50 @@ rnntStatus_t rnntb200_loss_device_fastemit(const float* activations, float* grad
                                            const int* label_lengths, const int* input_lengths, const float* grad_scale,
                                            int alphabet_size, int minibatch, float* costs_device, void* workspace,
                                            rnntOptions options, float fastemit_lambda) {
+    return rnntb200_loss_device_windowed(activations, gradients, flat_labels, label_lengths, input_lengths, grad_scale,
+                                         nullptr, nullptr, alphabet_size, minibatch, costs_device, workspace, options,
+                                         fastemit_lambda);
+}
+
+rnntStatus_t rnntb200_loss_device_windowed(const float* activations, float* gradients, const int* flat_labels,
+                                           const int* label_lengths, const int* input_lengths, const float* grad_scale,
+                                           const int* t_lo, const int* t_hi, int alphabet_size, int minibatch,
+                                           float* costs_device, void* workspace, rnntOptions options,
+                                           float fastemit_lambda) {
     if (!loss_args_ok(activations, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch, costs_device,
-                      workspace, options) || !fastemit_ok(fastemit_lambda))
+                      workspace, options) || !fastemit_ok(fastemit_lambda) || !windows_ok(t_lo, t_hi))
         return RNNT_STATUS_INVALID_VALUE;
+    const rb::Windows win{t_lo, t_hi};
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
     const bool vec = vec_ok<float>(activations, gradients, V);
     rnntStatus_t st = loss_forward(activations, vec, flat_labels, label_lengths, input_lengths, V, B, T, U, blank,
-                                   costs_device, workspace, s);
+                                   costs_device, workspace, s, win);
     if (st || !gradients) return st;
     return loss_grads<float, float>(activations, gradients, vec, flat_labels, label_lengths, input_lengths, grad_scale, V,
-                                    B, T, U, blank, workspace, s, fastemit_lambda);
+                                    B, T, U, blank, workspace, s, fastemit_lambda, win);
 }
 
 rnntStatus_t rnntb200_loss16_forward(const void* activations, int logit_type, const int* flat_labels,
                                      const int* label_lengths, const int* input_lengths, int alphabet_size, int minibatch,
                                      float* costs_device, void* workspace, rnntOptions options) {
+    return rnntb200_loss16_forward_windowed(activations, logit_type, flat_labels, label_lengths, input_lengths, nullptr,
+                                            nullptr, alphabet_size, minibatch, costs_device, workspace, options);
+}
+
+rnntStatus_t rnntb200_loss16_forward_windowed(const void* activations, int logit_type, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                              const int* t_hi, int alphabet_size, int minibatch, float* costs_device,
+                                              void* workspace, rnntOptions options) {
     if (!loss16_args_ok(activations, logit_type, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                        costs_device, workspace, options))
+                        costs_device, workspace, options) || !windows_ok(t_lo, t_hi))
         return RNNT_STATUS_INVALID_VALUE;
+    const rb::Windows win{t_lo, t_hi};
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
     return with_logits16(logit_type, activations, nullptr, [&](auto x, auto g) {
         return loss_forward(x, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, V, B, T, U, blank,
-                            costs_device, workspace, s);
+                            costs_device, workspace, s, win);
     });
 }
 
@@ -519,15 +553,26 @@ rnntStatus_t rnntb200_loss16_backward_fastemit(const void* activations, int logi
                                                const int* label_lengths, const int* input_lengths, const float* grad_costs,
                                                int alphabet_size, int minibatch, void* gradients, const void* workspace,
                                                rnntOptions options, float fastemit_lambda) {
+    return rnntb200_loss16_backward_windowed(activations, logit_type, flat_labels, label_lengths, input_lengths, nullptr,
+                                             nullptr, grad_costs, alphabet_size, minibatch, gradients, workspace, options,
+                                             fastemit_lambda);
+}
+
+rnntStatus_t rnntb200_loss16_backward_windowed(const void* activations, int logit_type, const int* flat_labels,
+                                               const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                               const int* t_hi, const float* grad_costs, int alphabet_size, int minibatch,
+                                               void* gradients, const void* workspace, rnntOptions options,
+                                               float fastemit_lambda) {
     if (!loss16_args_ok(activations, logit_type, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                        gradients, workspace, options) || !fastemit_ok(fastemit_lambda))
+                        gradients, workspace, options) || !fastemit_ok(fastemit_lambda) || !windows_ok(t_lo, t_hi))
         return RNNT_STATUS_INVALID_VALUE;
+    const rb::Windows win{t_lo, t_hi};
     cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
     const int V = alphabet_size, B = minibatch, T = options.maxT, U = options.maxU, blank = options.blank_label;
     void* ws = const_cast<void*>(workspace);      // read only: LossWs just carves the planes out of it
     return with_logits16(logit_type, activations, gradients, [&](auto x, auto g) {
         return loss_grads<float>(x, g, vec_ok<float>(x, g, V), flat_labels, label_lengths, input_lengths, grad_costs, V, B,
-                                 T, U, blank, ws, s, fastemit_lambda);
+                                 T, U, blank, ws, s, fastemit_lambda, win);
     });
 }
 
@@ -542,11 +587,20 @@ rnntStatus_t rnntb200_joint_loss_forward(const rnntb200JointDesc* desc, const fl
                                          const float* W, const float* bias, const int* labels,
                                          const int* label_lengths, const int* input_lengths, float* costs,
                                          void* workspace) {
-    if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !costs)
+    return rnntb200_joint_loss_forward_windowed(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, nullptr,
+                                                nullptr, costs, workspace);
+}
+
+rnntStatus_t rnntb200_joint_loss_forward_windowed(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                  const float* W, const float* bias, const int* labels,
+                                                  const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                                  const int* t_hi, float* costs, void* workspace) {
+    if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !costs ||
+        !windows_ok(t_lo, t_hi))
         return RNNT_STATUS_INVALID_VALUE;
     const int* overflow;
     return joint_forward(*desc, JointWs(*desc, workspace), enc, pred, W, bias, labels, label_lengths, input_lengths, costs,
-                         false, &overflow, reinterpret_cast<cudaStream_t>(desc->stream));
+                         false, &overflow, reinterpret_cast<cudaStream_t>(desc->stream), rb::Windows{t_lo, t_hi});
 }
 
 rnntStatus_t rnntb200_joint_loss_backward(const rnntb200JointDesc* desc, const float* enc, const float* pred,
@@ -563,20 +617,30 @@ rnntStatus_t rnntb200_joint_loss_backward_fastemit(const rnntb200JointDesc* desc
                                                    const int* label_lengths, const int* input_lengths,
                                                    const float* grad_costs, float* d_enc, float* d_pred, float* dW,
                                                    float* db, void* workspace, float fastemit_lambda) {
+    return rnntb200_joint_loss_backward_windowed(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, nullptr,
+                                                 nullptr, grad_costs, d_enc, d_pred, dW, db, workspace, fastemit_lambda);
+}
+
+rnntStatus_t rnntb200_joint_loss_backward_windowed(const rnntb200JointDesc* desc, const float* enc, const float* pred,
+                                                   const float* W, const float* bias, const int* labels,
+                                                   const int* label_lengths, const int* input_lengths, const int* t_lo,
+                                                   const int* t_hi, const float* grad_costs, float* d_enc, float* d_pred,
+                                                   float* dW, float* db, void* workspace, float fastemit_lambda) {
     if (!joint_loss_args_ok(desc, enc, pred, W, bias, labels, label_lengths, input_lengths, workspace) || !grad_costs ||
-        !d_enc || !d_pred || !dW || !db || !fastemit_ok(fastemit_lambda))
+        !d_enc || !d_pred || !dW || !db || !fastemit_ok(fastemit_lambda) || !windows_ok(t_lo, t_hi))
         return RNNT_STATUS_INVALID_VALUE;
+    const rb::Windows win{t_lo, t_hi};
     const rnntb200JointDesc& d = *desc;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(d.stream);
     JointWs ws(d, workspace);
     if (d.precision == RNNTB200_FP32_EXACT)
         return exact_backward(d, ws, enc, pred, W, bias, labels, label_lengths, input_lengths, grad_costs, d_enc,
-                              d_pred, dW, db, s, fastemit_lambda);
+                              d_pred, dW, db, s, fastemit_lambda, win);
 #ifndef RNNTB200_NO_TC
     unsigned nl = 0;
     const rb::LossPlanes lp{ws.loss.lse, ws.loss.lpb, ws.loss.lpl, ws.loss.alphas, ws.loss.betas, ws.loss.llf};
     rnntStatus_t st = rb::tc_backward(d, ws.scratch, enc, pred, bias, labels, label_lengths, input_lengths, lp, grad_costs,
-                                      d_enc, d_pred, dW, db, s, &nl, fastemit_lambda);
+                                      d_enc, d_pred, dW, db, s, &nl, fastemit_lambda, win);
     RB_LAUNCHED(nl);
     return st;
 #else

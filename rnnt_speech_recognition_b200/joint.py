@@ -17,19 +17,13 @@ import torch
 
 from . import _lib
 from .loss import encoder_lengths
+from .windows import check_windows, valid_tile_count
 
 __all__ = ["joint_rnnt_loss", "joint_logits", "joint_step", "Joint", "get_fused_loss_fn"]
 
 _PREC = {"fp32": _lib.FP32_EXACT, "bf16": _lib.BF16_TC, _lib.FP32_EXACT: _lib.FP32_EXACT, _lib.BF16_TC: _lib.BF16_TC}
 
 _ptr = _lib.ptr
-
-
-def valid_tile_count(input_lengths, label_lengths):
-    """Number of 16 x 8 lattice tiles that intersect the valid lattices of a batch, from HOST copies of the lengths (lists,
-    numpy arrays or CPU tensors): the value `joint_rnnt_loss(..., valid_tiles=...)` / `rnntb200JointDesc.valid_tile_bound`
-    expects.  A data loader has the lengths on the host anyway; the library itself never reads device memory back."""
-    return int(sum(((int(t) + 15) // 16) * ((int(u) + 1 + 7) // 8) for t, u in zip(input_lengths, label_lengths)))
 
 
 def _desc(B, T, U, H, V, blank, precision, keep=False, tile_bound=0):
@@ -92,7 +86,7 @@ def _joint_setup(enc, pred, W, b, labels, input_lengths, label_lengths, blank, p
 class _JointRNNT(torch.autograd.Function):
     @staticmethod
     def forward(ctx, enc, pred, W, b, labels, input_lengths, label_lengths, blank, precision, compact, keep=None, valid_tiles=None,
-                fastemit_lambda=0.0):
+                fastemit_lambda=0.0, t_lo=None, t_hi=None):
         L = _lib.load()
         # a backward will follow: let the forward keep its softmax numerators / tanh outputs in the workspace
         keep = any(ctx.needs_input_grad[:4]) if keep is None else keep
@@ -101,9 +95,11 @@ class _JointRNNT(torch.autograd.Function):
         device = args[0].device
         costs = torch.empty(desc.B, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            st = L.rnntb200_joint_loss_forward(C.byref(desc), *map(_ptr, args), _ptr(costs), _ptr(ws))
-        _lib.check(st, "rnntb200_joint_loss_forward")
+            st = L.rnntb200_joint_loss_forward_windowed(C.byref(desc), *map(_ptr, args), _ptr(t_lo), _ptr(t_hi), _ptr(costs),
+                                                        _ptr(ws))
+        _lib.check(st, "rnntb200_joint_loss_forward_windowed")
         ctx.save_for_backward(*args)
+        ctx.windows = (t_lo, t_hi)
         ctx.ws, ctx.desc, ctx.fastemit_lambda = ws, desc, fastemit_lambda
         return costs
 
@@ -116,15 +112,16 @@ class _JointRNNT(torch.autograd.Function):
         with torch.cuda.device(args[0].device):
             desc = ctx.desc
             desc.stream = _lib.stream().value          # the forward's descriptor, on the backward's current stream
-            st = L.rnntb200_joint_loss_backward_fastemit(C.byref(desc), *map(_ptr, args), _ptr(g), _ptr(d_enc),
-                                                         _ptr(d_pred), _ptr(dW), _ptr(db), _ptr(ctx.ws), ctx.fastemit_lambda)
-        _lib.check(st, "rnntb200_joint_loss_backward_fastemit")
+            st = L.rnntb200_joint_loss_backward_windowed(C.byref(desc), *map(_ptr, args), *map(_ptr, ctx.windows), _ptr(g),
+                                                         _ptr(d_enc), _ptr(d_pred), _ptr(dW), _ptr(db), _ptr(ctx.ws),
+                                                         ctx.fastemit_lambda)
+        _lib.check(st, "rnntb200_joint_loss_backward_windowed")
         ctx.ws = None
-        return d_enc, d_pred, dW, db, None, None, None, None, None, None, None, None, None
+        return (d_enc, d_pred, dW, db) + (None,) * 11
 
 
 def joint_rnnt_loss(enc_acts, pred_acts, W, b, labels, input_lengths, label_lengths, blank=0, precision="bf16",
-                    compact=True, keep_activations=None, valid_tiles=None, fastemit_lambda=0.0):
+                    compact=True, keep_activations=None, valid_tiles=None, fastemit_lambda=0.0, windows=None):
     """Per-utterance RNN-T NLL (B,) of logits = tanh(enc_acts[:,:,None]+pred_acts[:,None]) @ W + b,
     differentiable w.r.t. enc_acts, pred_acts, W, b -- without ever materialising (B,T,U,V).
     precision: 'bf16' = the tensor-core path (wgmma, 16-bit operands, fp32 accumulate) or 'fp32' (exact CUDA-core path).
@@ -140,10 +137,15 @@ def joint_rnnt_loss(enc_acts, pred_acts, W, b, labels, input_lengths, label_leng
     float16 / bfloat16 inputs are cast to float32 first (costs float32, each gradient in its input's dtype).
     fastemit_lambda: FastEmit regularisation (Yu et al. 2021), a finite float >= 0 (ValueError otherwise): the gradient
     of every label-emission log-probability is scaled by (1 + lambda); the costs stay -log p(y|x).  0 = the plain loss,
-    bit for bit."""
+    bit for bit.
+    windows: optional ``(t_lo, t_hi)``, int32 CUDA tensors (B, U): the alignment-restricted loss (windows.py), summed over
+    the paths inside the per-column frame windows only; lattice tiles outside them are never computed.  With windows,
+    ``valid_tiles`` is ``valid_tile_count(host lengths, windows=host windows)``: the workspace then holds the band only.
+    Windows that admit no path give a cost of +inf and zero gradients; full windows are the plain loss, bit for bit."""
     lam = _lib.fastemit_lambda(fastemit_lambda)
+    t_lo, t_hi = check_windows(windows, enc_acts.shape[0], pred_acts.shape[1], enc_acts.device)
     return _JointRNNT.apply(_f32(enc_acts), _f32(pred_acts), _f32(W), _f32(b), labels, input_lengths, label_lengths, blank,
-                            precision, compact, keep_activations, valid_tiles, lam)
+                            precision, compact, keep_activations, valid_tiles, lam, t_lo, t_hi)
 
 
 def joint_logits(enc_acts, pred_acts, W, b):
@@ -283,10 +285,12 @@ class Joint(torch.nn.Module):
                                    want_logits=False, want_best=True)
         return best, logp
 
-    def loss(self, inp_enc, pred_outputs, labels, input_lengths, label_lengths):
+    def loss(self, inp_enc, pred_outputs, labels, input_lengths, label_lengths, windows=None, valid_tiles=None):
+        """``windows`` / ``valid_tiles``: the alignment-restricted loss, as in ``joint_rnnt_loss``."""
         enc_acts, pred_acts = self.hoist(inp_enc, pred_outputs)
         return joint_rnnt_loss(enc_acts, pred_acts, self.kernel_2, self.bias_2, labels, input_lengths, label_lengths,
-                               self.blank, self.precision, fastemit_lambda=self.fastemit_lambda)
+                               self.blank, self.precision, valid_tiles=valid_tiles, fastemit_lambda=self.fastemit_lambda,
+                               windows=windows)
 
     @torch.no_grad()
     def align(self, inp_enc, pred_outputs, labels, input_lengths, label_lengths):
@@ -304,9 +308,10 @@ def get_fused_loss_fn(reduction_factor, joint):
     network's INPUTS in place of y_pred (run_rnnt.py:269-273 collapsed into one call)."""
     _lib.load()
 
-    def _loss_fn(y_true, inp_enc, pred_outputs, spec_lengths, label_lengths):
+    def _loss_fn(y_true, inp_enc, pred_outputs, spec_lengths, label_lengths, windows=None):
         y_true = y_true.to(torch.int32).contiguous()
         enc_lengths = encoder_lengths(spec_lengths, reduction_factor).contiguous()
-        return joint.loss(inp_enc, pred_outputs, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous())
+        kw = {} if windows is None else {"windows": windows}
+        return joint.loss(inp_enc, pred_outputs, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous(), **kw)
 
     return _loss_fn

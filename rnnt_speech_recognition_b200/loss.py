@@ -22,12 +22,14 @@ def get_loss_fn(reduction_factor, fastemit_lambda=0.0):
     lam = _lib.fastemit_lambda(fastemit_lambda)
     _lib.load()  # fail loudly here, not with a fallback later
 
-    def _loss_fn(y_true, y_pred, spec_lengths, label_lengths):
+    def _loss_fn(y_true, y_pred, spec_lengths, label_lengths, windows=None):
         """y_true (B,U-1) int labels; y_pred (B,T,U,V) float32 / float16 / bfloat16 logits; spec_lengths (B,) pre-reduction
-        frame counts; label_lengths (B,) -> per-utterance NLL (B,).  utils/loss.py:24-36."""
+        frame counts; label_lengths (B,) -> per-utterance NLL (B,).  utils/loss.py:24-36.  windows: optional (t_lo, t_hi) of
+        the alignment-restricted loss (``rnnt_loss``)."""
         y_true = y_true.to(torch.int32).contiguous()                 # tf.cast(y_true, tf.int32)
         # GPU build: no explicit log_softmax (utils/loss.py:29-30 applies it only on CPU builds)
         enc_lengths = encoder_lengths(spec_lengths, reduction_factor).contiguous()
-        return rnnt_loss(y_pred, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous(), fastemit_lambda=lam)
+        return rnnt_loss(y_pred, y_true, enc_lengths, label_lengths.to(torch.int32).contiguous(), fastemit_lambda=lam,
+                         windows=windows)
 
     return _loss_fn

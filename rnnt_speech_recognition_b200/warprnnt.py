@@ -24,6 +24,7 @@ import ctypes as C
 import torch
 
 from . import _lib
+from .windows import check_windows
 
 __all__ = ["rnnt_loss", "torch_rnnt_loss", "RNNTLoss", "certify_inputs"]
 
@@ -107,16 +108,16 @@ class _RNNTOp(torch.autograd.Function):
     as both reference bindings do (warprnnt_op.cc:100-137, warprnnt_pytorch/__init__.py:24-42)."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0, t_lo=None, t_hi=None):
         L = _lib.load()
         (B, T, U, V), ws, lab = _prepare(acts, labels, act_lens, label_lens, float32_only=True)
         grads = torch.empty_like(acts) if acts.requires_grad else None
         costs = torch.empty(B, dtype=torch.float32, device=acts.device)
         with torch.cuda.device(acts.device):
-            st = L.rnntb200_loss_device_fastemit(_ptr(acts), _ptr(grads), _ptr(lab), _ptr(label_lens), _ptr(act_lens),
-                                                 None, V, B, _ptr(costs), _ptr(ws), _options(blank, T, U),
-                                                 fastemit_lambda)
-        _lib.check(st, "rnntb200_loss_device_fastemit")
+            st = L.rnntb200_loss_device_windowed(_ptr(acts), _ptr(grads), _ptr(lab), _ptr(label_lens), _ptr(act_lens),
+                                                 None, _ptr(t_lo), _ptr(t_hi), V, B, _ptr(costs), _ptr(ws),
+                                                 _options(blank, T, U), fastemit_lambda)
+        _lib.check(st, "rnntb200_loss_device_windowed")
         ctx.grads = grads
         return costs
 
@@ -124,7 +125,7 @@ class _RNNTOp(torch.autograd.Function):
     def backward(ctx, grad_costs):
         g = ctx.grads
         ctx.grads = None
-        return g.mul_(grad_costs.view(-1, 1, 1, 1).to(g)), None, None, None, None, None
+        return (g.mul_(grad_costs.view(-1, 1, 1, 1).to(g)),) + (None,) * 7
 
 
 _LOGIT_TYPE = {torch.float16: _lib.LOGITS_F16, torch.bfloat16: _lib.LOGITS_BF16}
@@ -136,15 +137,17 @@ class _RNNTOp16(torch.autograd.Function):
     single rounding, so a loss-scaled fp16 gradient does not underflow and no fp32 (B,T,U,V) tensor ever exists."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, fastemit_lambda=0.0, t_lo=None, t_hi=None):
         L = _lib.load()
         (B, T, U, V), ws, lab = _prepare(acts, labels, act_lens, label_lens)
         costs = torch.empty(B, dtype=torch.float32, device=acts.device)
         with torch.cuda.device(acts.device):
-            st = L.rnntb200_loss16_forward(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
-                                           _ptr(act_lens), V, B, _ptr(costs), _ptr(ws), _options(blank, T, U))
-        _lib.check(st, "rnntb200_loss16_forward")
+            st = L.rnntb200_loss16_forward_windowed(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
+                                                    _ptr(act_lens), _ptr(t_lo), _ptr(t_hi), V, B, _ptr(costs), _ptr(ws),
+                                                    _options(blank, T, U))
+        _lib.check(st, "rnntb200_loss16_forward_windowed")
         if acts.requires_grad:
+            ctx.windows = (t_lo, t_hi)
             ctx.save_for_backward(acts, lab, act_lens, label_lens)
             ctx.ws, ctx.blank, ctx.fastemit_lambda = ws, int(blank), fastemit_lambda
         return costs
@@ -158,12 +161,12 @@ class _RNNTOp16(torch.autograd.Function):
         g = grad_costs.to(torch.float32).contiguous()
         grads = torch.empty_like(acts)
         with torch.cuda.device(acts.device):
-            st = L.rnntb200_loss16_backward_fastemit(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
-                                                     _ptr(act_lens), _ptr(g), V, B, _ptr(grads), _ptr(ctx.ws),
-                                                     _options(ctx.blank, T, U), ctx.fastemit_lambda)
-        _lib.check(st, "rnntb200_loss16_backward_fastemit")
+            st = L.rnntb200_loss16_backward_windowed(_ptr(acts), _LOGIT_TYPE[acts.dtype], _ptr(lab), _ptr(label_lens),
+                                                     _ptr(act_lens), *map(_ptr, ctx.windows), _ptr(g), V, B, _ptr(grads),
+                                                     _ptr(ctx.ws), _options(ctx.blank, T, U), ctx.fastemit_lambda)
+        _lib.check(st, "rnntb200_loss16_backward_windowed")
         ctx.ws = None
-        return grads, None, None, None, None, None
+        return (grads,) + (None,) * 7
 
 
 def _op(acts):
@@ -171,25 +174,29 @@ def _op(acts):
     return _RNNTOp16 if acts.dtype in _LOGIT_TYPE else _RNNTOp
 
 
-def rnnt_loss(acts, labels, input_lengths, label_lengths, blank_label=0, fastemit_lambda=0.0):
+def rnnt_loss(acts, labels, input_lengths, label_lengths, blank_label=0, fastemit_lambda=0.0, windows=None):
     """TF-binding signature (warprnnt_tensorflow/__init__.py:9): per-utterance costs (B,).
     ``acts`` are raw logits (B,T,U,V) float32, float16 or bfloat16 -- the softmax is performed inside, as the
     reference's GPU op does; costs are float32 and ``acts.grad`` has ``acts.dtype``.  ``labels`` (B,U-1) int32 zero
     padded; lengths (B,) int32.  ``fastemit_lambda`` >= 0 (finite; ValueError otherwise): FastEmit regularisation of
-    the gradient, costs unchanged."""
+    the gradient, costs unchanged.  ``windows``: optional ``(t_lo, t_hi)`` int32 CUDA tensors (B,U), the
+    alignment-restricted loss (windows.py): only paths inside the per-column frame windows count, the gradients of cells
+    outside them are exactly 0 and their logits are not read; windows that admit no path give a cost of +inf."""
     lam = _lib.fastemit_lambda(fastemit_lambda)
     acts = acts.contiguous()
     certify_inputs(acts, labels, input_lengths, label_lengths, check_max=False)
-    return _op(acts).apply(acts, labels, input_lengths, label_lengths, blank_label, lam)
+    t_lo, t_hi = check_windows(windows, acts.shape[0], acts.shape[2], acts.device)
+    return _op(acts).apply(acts, labels, input_lengths, label_lengths, blank_label, lam, t_lo, t_hi)
 
 
-def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean", fastemit_lambda=0.0):
+def torch_rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction="mean", fastemit_lambda=0.0, windows=None):
     """warprnnt_pytorch.rnnt_loss (pytorch_binding/warprnnt_pytorch/__init__.py:53-70):
     reduction in {'none','sum','mean'}; 'mean' divides the summed cost by the batch size.  ``acts`` float32, float16
-    or bfloat16 (costs float32 either way).  ``fastemit_lambda``: as in ``rnnt_loss``."""
+    or bfloat16 (costs float32 either way).  ``fastemit_lambda``, ``windows``: as in ``rnnt_loss``."""
     lam = _lib.fastemit_lambda(fastemit_lambda)
     certify_inputs(acts, labels, act_lens, label_lens, check_max=True)
-    costs = _op(acts).apply(acts, labels, act_lens, label_lens, blank, lam)
+    t_lo, t_hi = check_windows(windows, acts.shape[0], acts.shape[2], acts.device)
+    costs = _op(acts).apply(acts, labels, act_lens, label_lens, blank, lam, t_lo, t_hi)
     if reduction in ("sum", "mean"):
         costs = costs.sum().unsqueeze(-1)
         if reduction == "mean":
@@ -208,5 +215,6 @@ class RNNTLoss(torch.nn.Module):
         self.reduction = reduction
         self.fastemit_lambda = _lib.fastemit_lambda(fastemit_lambda)
 
-    def forward(self, acts, labels, act_lens, label_lens):
-        return torch_rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda)
+    def forward(self, acts, labels, act_lens, label_lens, windows=None):
+        return torch_rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda,
+                               windows)
