@@ -367,6 +367,49 @@ rnntStatus_t rnntb200_dense1_forward(const float* X, long long rows, int P, cons
 rnntStatus_t rnntb200_dense1_backward(const float* X, const float* dA, const float* K1, long long rows, int P, int H,
                                       float* dX, float* dK1, float* db1, CUstream stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Part 3 -- pruned RNN-T (Kuang, Guo, Kang, Lin, Povey, "Pruned RNN-T for fast, memory-efficient ASR training",
+ * Interspeech 2022): the trivial joiner's "simple" loss and the band it chooses for the full joint
+ * ------------------------------------------------------------------------------------------ */
+
+/** The simple loss: am (B,maxT,V) and lm (B,maxU,V) fp32 device, row-major; labels (B,maxU-1), label_lengths (B),
+ *  input_lengths (B) int32 device; options.blank_label / maxT / maxU / stream as in rnntb200_loss16_forward (loc and
+ *  num_threads are ignored).  The cost is the ordinary RNN-T loss, softmax inside, over the logits
+ *    x[b,t,u,:] = am[b,t,:] + lm[b,u,:]
+ *  i.e. rnntb200_loss_device on am[:,:,None,:] + lm[:,None,:,:], without that (B,T,U,V) tensor ever being formed: the
+ *  log-softmax normaliser factorises into exp(am - max) . exp(lm - max)^T, an fp32 FMA GEMM per utterance.  A cell whose
+ *  factorised normaliser falls below 2^-64 (am's and lm's large entries in different columns) takes a direct log-sum-exp
+ *  over V instead, and its exact softmax in the backward: costs stay finite however far apart the two peaks are.
+ *  Workspace: rnntb200_simple_workspace_size bytes (a pure function).  No FastEmit and no windows on this loss.
+ *  Stream-ordered, no allocation, no host synchronisation, CUDA-graph capturable; no float atomics (bit-identical reruns).
+ *  Errors: NULL pointers, non-positive sizes, maxU > 1024 or a blank outside [0, V) -> RNNT_STATUS_INVALID_VALUE before
+ *  any device work. */
+rnntStatus_t rnntb200_simple_workspace_size(int B, int maxT, int maxU, int V, size_t* size_bytes);
+
+/** Forward: costs (B) fp32 DEVICE, -log p(y|x) of the simple lattice; leaves its planes in the workspace. */
+rnntStatus_t rnntb200_simple_loss_forward(const float* am, const float* lm, const int* labels, const int* label_lengths,
+                                          const int* input_lengths, int V, int B, float* costs, void* workspace,
+                                          rnntOptions options);
+
+/** Backward on the forward's unchanged workspace (which it leaves unchanged for the windows call):
+ *  d_am[b,t,:] = sum_u grad_costs[b] dx[b,t,u,:] and d_lm[b,u,:] = sum_t grad_costs[b] dx[b,t,u,:], fp32 device,
+ *  OVERWRITTEN; rows at t >= T_b or u >= U_b are exactly 0.  grad_costs: optional DEVICE float (B), NULL means 1. */
+rnntStatus_t rnntb200_simple_loss_backward(const float* am, const float* lm, const int* labels, const int* label_lengths,
+                                           const int* input_lengths, int V, int B, const float* grad_costs, float* d_am,
+                                           float* d_lm, void* workspace, rnntOptions options);
+
+/** The pruning band of the forward's simple lattice (DESIGN §1), as the per-column frame windows of the _windowed entries:
+ *  with S = s_range >= 2 and gamma_B / gamma_L the blank- and label-arc occupancies,
+ *    score(t,s) = sum_{u=s}^{min(s+S,U_b)-1} gamma_B(t,u) - gamma_L(t,s-1),  s in [0, max(0, U_b - S)];
+ *  s_t its smallest argmax for t < T_b - 1 and s_{T_b-1} = max(0, U_b - S); then s_t <- min_{t' >= t} s_t' and
+ *  s_t <- min((S-1) t, max_{t' >= t} (s_t' - (S-1)(t' - t))).  Cell (t,u) is in the band iff s_t <= u < s_t + S, and
+ *    t_lo[b,u] = min{t < T_b : s_t <= u < s_t + S},  t_hi[b,u] = max{...}   (int32 DEVICE (B, maxU)),
+ *  (0, -1) for u >= U_b and for a column no frame's band reaches.  The band admits a path iff (S-1) T_b >= U_b - 1;
+ *  S >= U_b gives full windows.  Reads the forward's planes and does not modify them; uses the workspace's own band
+ *  planes.  Errors: NULL pointers, B <= 0, s_range < 2, maxU > 1024 -> RNNT_STATUS_INVALID_VALUE. */
+rnntStatus_t rnntb200_simple_prune_windows(const int* label_lengths, const int* input_lengths, int B, int s_range,
+                                           int* t_lo, int* t_hi, void* workspace, rnntOptions options);
+
 /** Number of kernels launched by this library in this process since load (bench.py's gpu_launches).  Every kernel
  *  on the path is the library's own: it links no GEMM library. */
 unsigned long long rnntb200_launch_count();

@@ -37,6 +37,8 @@ EXPORTS = ("get_warprnnt_version", "rnntGetStatusString", "get_workspace_size", 
            "rnntb200_align_device", "rnntb200_align16", "rnntb200_joint_align",
            "rnntb200_joint_logits", "rnntb200_joint_step",
            "rnntb200_dense1_forward", "rnntb200_dense1_backward",
+           "rnntb200_simple_workspace_size", "rnntb200_simple_loss_forward", "rnntb200_simple_loss_backward",
+           "rnntb200_simple_prune_windows",
            "rnntb200_launch_count", "rnntb200_build_info", "rnntb200_set_timing", "rnntb200_get_timing")
 
 _lib = None
@@ -89,6 +91,10 @@ def load(build_if_missing=True):
     L.rnntb200_joint_step.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
     L.rnntb200_dense1_forward.argtypes = [vp, C.c_longlong, ci, vp, vp, ci, vp, vp]
     L.rnntb200_dense1_backward.argtypes = [vp, vp, vp, C.c_longlong, ci, ci, vp, vp, vp, vp]
+    L.rnntb200_simple_workspace_size.argtypes = [ci, ci, ci, ci, C.POINTER(C.c_size_t)]
+    L.rnntb200_simple_loss_forward.argtypes = [vp] * 5 + [ci, ci, vp, vp, RnntOptions]
+    L.rnntb200_simple_loss_backward.argtypes = [vp] * 5 + [ci, ci, vp, vp, vp, vp, RnntOptions]
+    L.rnntb200_simple_prune_windows.argtypes = [vp, vp, ci, ci, vp, vp, vp, RnntOptions]
     L.rnntb200_launch_count.restype = C.c_ulonglong
     L.rnntb200_build_info.restype = C.c_char_p
     L.rnntb200_set_timing.argtypes = [ci]

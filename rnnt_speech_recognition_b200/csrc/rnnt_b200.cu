@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 
 #include "kernels_simt.cuh"
+#include "simple_joiner.cuh"
 #include "timing.cuh"
 #include "joint_step.cuh"
 #ifndef RNNTB200_NO_TC
@@ -439,6 +440,56 @@ bool joint_loss_args_ok(const rnntb200JointDesc* d, const float* enc, const floa
     return desc_ok(d) && enc && pred && W && bias && labels && ylen && xlen && workspace;
 }
 
+// ------------------------------------------------------------------------------------------
+// simple (trivial-joiner) loss of pruned RNN-T (csrc/simple_joiner.cuh)
+// ------------------------------------------------------------------------------------------
+// Workspace: the loss op's planes (LossWs), the row maxima, Ea / El, the normaliser plane (forward), the G plane
+// (backward), the underflow flags and the two band planes of the windows call.  Each call writes only its own parts, so
+// the backward and the windows call leave what the forward wrote unchanged.  Ea / El come last: the windows call has no V
+// and locates everything else with V = 0.
+struct SimpleWs {
+    LossWs<float> loss;
+    float *ma, *ml, *nrm, *G, *Ea, *El;
+    unsigned char* flag;
+    int *s_raw, *s_band;
+    size_t total;
+    SimpleWs(void* base, int B, int maxT, int maxU, int V) : loss(base, B, maxT, maxU) {
+        const size_t NT = (size_t)B * maxT, NU = (size_t)B * maxU, N = NT * maxU;
+        char* p = static_cast<char*>(base);
+        size_t off = align_up(loss.bytes, 256);
+        auto take = [&](size_t bytes) { char* q = p + off; off += align_up(bytes, 256); return q; };
+        ma = reinterpret_cast<float*>(take(NT * 4));
+        ml = reinterpret_cast<float*>(take(NU * 4));
+        nrm = reinterpret_cast<float*>(take(N * 4));
+        G = reinterpret_cast<float*>(take(N * 4));
+        flag = reinterpret_cast<unsigned char*>(take(N));
+        s_raw = reinterpret_cast<int*>(take(NT * 4));
+        s_band = reinterpret_cast<int*>(take(NT * 4));
+        Ea = reinterpret_cast<float*>(take(NT * V * 4));
+        El = reinterpret_cast<float*>(take(NU * V * 4));
+        total = off;
+    }
+};
+
+bool simple_args_ok(const float* am, const float* lm, const int* labels, const int* ylen, const int* xlen, int V, int B,
+                    const void* workspace, const rnntOptions& o) {
+    return am && lm && labels && ylen && xlen && workspace && V > 0 && B > 0 && o.maxT > 0 && o.maxU > 0 &&
+           o.maxU <= 1024 && o.blank_label >= 0 && o.blank_label < V;
+}
+
+// C[b] (M x N) = A[b] . B[b] (EPI 0) or X[b] (.) (A[b] . B[b]) (EPI 1), one launch per 65535 batches
+template <bool AK, bool BN, int EPI>
+void launch_bgemm(const float* A, const float* Bm, float* C, const float* X, int M, int N, int K, long long sA, long long sB,
+                  long long ldc, long long bA, long long bB, long long bC, int batches, cudaStream_t s) {
+    for (int b0 = 0; b0 < batches; b0 += 65535) {
+        const int nb = min(65535, batches - b0);
+        dim3 grid((N + 127) / 128, (M + 127) / 128, nb);
+        rb::bgemm_kernel<AK, BN, EPI><<<grid, 256, 0, s>>>(A + b0 * bA, Bm + b0 * bB, C + b0 * bC, EPI ? X + b0 * bC : nullptr,
+                                                           M, N, K, sA, sB, ldc, bA, bB, bC);
+        RB_LAUNCHED(1);
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -758,6 +809,111 @@ rnntStatus_t rnntb200_dense1_backward(const float* X, const float* dA, const flo
         rb::colsum_kernel<<<dim3((H + 31) / 32, 1), 256, 0, s>>>(dA, rows, H, db1);      // one row block: deterministic
         RB_LAUNCHED(1);
     }
+    return check_launch();
+}
+
+rnntStatus_t rnntb200_simple_workspace_size(int B, int maxT, int maxU, int V, size_t* size_bytes) {
+    if (B <= 0 || maxT <= 0 || maxU <= 0 || maxU > 1024 || V <= 0 || !size_bytes) return RNNT_STATUS_INVALID_VALUE;
+    *size_bytes = SimpleWs(nullptr, B, maxT, maxU, V).total;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnntb200_simple_loss_forward(const float* am, const float* lm, const int* labels, const int* label_lengths,
+                                          const int* input_lengths, int V, int B, float* costs, void* workspace,
+                                          rnntOptions options) {
+    if (!simple_args_ok(am, lm, labels, label_lengths, input_lengths, V, B, workspace, options) || !costs)
+        return RNNT_STATUS_INVALID_VALUE;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
+    const int T = options.maxT, U = options.maxU, blank = options.blank_label;
+    const SimpleWs w(workspace, B, T, U, V);
+    const long long NT = (long long)B * T, NU = (long long)B * U, N = NT * U, SK = skew_plane(T, U);
+    {
+        rb::ScopedTimer tm("simple_exp_rows_kernel", s);
+        rb::simple_exp_rows_kernel<<<(unsigned)((NT * 32 + 255) / 256), 256, 0, s>>>(am, NT, T, V, input_lengths, 0, w.ma, w.Ea);
+        rb::simple_exp_rows_kernel<<<(unsigned)((NU * 32 + 255) / 256), 256, 0, s>>>(lm, NU, U, V, label_lengths, 1, w.ml, w.El);
+    }
+    RB_LAUNCHED(2);
+    {   // Nrm[b] = Ea[b] . El[b]^T:  A(t,v) = Ea[t*V + v],  B(v,u) = El[u*V + v]
+        rb::ScopedTimer tm("bgemm Nrm=Ea.El^T", s);
+        launch_bgemm<true, false, 0>(w.Ea, w.El, w.nrm, nullptr, T, U, V, V, V, U, (long long)T * V, (long long)U * V,
+                                     (long long)T * U, B, s);
+    }
+    {
+        rb::ScopedTimer tm("simple_lse_kernel", s);
+        rb::simple_lse_kernel<<<(unsigned)((N * 32 + 255) / 256), 256, 0, s>>>(am, lm, w.ma, w.ml, w.nrm, input_lengths,
+                                                                            label_lengths, labels, T, U, SK, N, V, blank,
+                                                                            w.loss.lse, w.loss.lpb, w.loss.lpl, w.flag);
+    }
+    RB_LAUNCHED(1);
+    if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
+    if (launch_alpha_beta(w.loss, input_lengths, label_lengths, B, T, U, s)) return RNNT_STATUS_EXECUTION_FAILED;
+    return launch_finish_costs(w.loss.llf, w.loss.llb, costs, B, nullptr, s);
+}
+
+rnntStatus_t rnntb200_simple_loss_backward(const float* am, const float* lm, const int* labels, const int* label_lengths,
+                                           const int* input_lengths, int V, int B, const float* grad_costs, float* d_am,
+                                           float* d_lm, void* workspace, rnntOptions options) {
+    if (!simple_args_ok(am, lm, labels, label_lengths, input_lengths, V, B, workspace, options) || !d_am || !d_lm)
+        return RNNT_STATUS_INVALID_VALUE;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
+    const int T = options.maxT, U = options.maxU, blank = options.blank_label;
+    const SimpleWs w(workspace, B, T, U, V);
+    const LossWs<float>& L = w.loss;
+    const long long N = (long long)B * T * U, SK = skew_plane(T, U);
+    {
+        rb::ScopedTimer tm("simple_g_kernel", s);
+        rb::simple_g_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(w.ma, w.ml, L.lse, L.alphas, L.betas, L.llf, w.flag,
+                                                                       grad_costs, input_lengths, label_lengths, T, U, SK,
+                                                                       N, w.G);
+    }
+    RB_LAUNCHED(1);
+    {   // d_am[b] = Ea[b] (.) (G[b] . El[b]):  A(t,u) = G[t*U + u],  B(u,v) = El[u*V + v]
+        rb::ScopedTimer tm("bgemm d_am=Ea*(G.El)", s);
+        launch_bgemm<true, true, 1>(w.G, w.El, d_am, w.Ea, T, V, U, U, V, V, (long long)T * U, (long long)U * V,
+                                    (long long)T * V, B, s);
+    }
+    {   // d_lm[b] = El[b] (.) (G[b]^T . Ea[b]):  A(u,t) = G[t*U + u],  B(t,v) = Ea[t*V + v]
+        rb::ScopedTimer tm("bgemm d_lm=El*(G^T.Ea)", s);
+        launch_bgemm<false, true, 1>(w.G, w.Ea, d_lm, w.El, U, V, T, U, V, V, (long long)T * U, (long long)T * V,
+                                     (long long)U * V, B, s);
+    }
+    if (check_launch()) return RNNT_STATUS_EXECUTION_FAILED;
+    {
+        rb::ScopedTimer tm("simple_dam_fix_kernel", s);
+        rb::simple_dam_fix_kernel<<<(unsigned)(B * T), rb::SIMPLE_FIX_THREADS, 0, s>>>(
+            am, lm, L.lse, L.lpb, L.lpl, L.alphas, L.betas, L.llf, w.flag, grad_costs, input_lengths, label_lengths, labels,
+            T, U, SK, V, blank, d_am);
+    }
+    {
+        rb::ScopedTimer tm("simple_dlm_fix_kernel", s);
+        rb::simple_dlm_fix_kernel<<<(unsigned)(B * U), rb::SIMPLE_FIX_THREADS, 0, s>>>(
+            am, lm, L.lse, L.lpb, L.lpl, L.alphas, L.betas, L.llf, w.flag, grad_costs, input_lengths, label_lengths, labels,
+            T, U, SK, V, blank, d_lm);
+    }
+    RB_LAUNCHED(2);
+    return check_launch();
+}
+
+rnntStatus_t rnntb200_simple_prune_windows(const int* label_lengths, const int* input_lengths, int B, int s_range,
+                                           int* t_lo, int* t_hi, void* workspace, rnntOptions options) {
+    if (!label_lengths || !input_lengths || !t_lo || !t_hi || !workspace || B <= 0 || s_range < 2 || options.maxT <= 0 ||
+        options.maxU <= 0 || options.maxU > 1024)
+        return RNNT_STATUS_INVALID_VALUE;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(options.stream);
+    const int T = options.maxT, U = options.maxU;
+    const SimpleWs w(workspace, B, T, U, 0);
+    const LossWs<float>& L = w.loss;
+    {
+        rb::ScopedTimer tm("prune_score_kernel", s);
+        rb::prune_score_kernel<<<dim3(B, (T + rb::PRUNE_WARPS - 1) / rb::PRUNE_WARPS), rb::PRUNE_WARPS * 32, 0, s>>>(
+            L.lpb, L.lpl, L.alphas, L.betas, L.llf, input_lengths, label_lengths, T, U, skew_plane(T, U), s_range, w.s_raw);
+    }
+    {
+        rb::ScopedTimer tm("prune_windows_kernel", s);
+        rb::prune_windows_kernel<<<B, rb::PRUNE_THREADS, 0, s>>>(w.s_raw, w.s_band, input_lengths, label_lengths, T, U,
+                                                                 s_range, t_lo, t_hi);
+    }
+    RB_LAUNCHED(2);
     return check_launch();
 }
 
