@@ -213,7 +213,10 @@ typedef struct {
     int keep_activations;
 } rnntb200JointDesc;
 
-/** Bytes of device workspace the forward/backward pair needs (pure function of the descriptor). */
+/** Bytes of device workspace the forward/backward pair needs (pure function of the descriptor).  On the tensor-core
+ *  path this includes, besides the kept numerators the chunk plan is sized by, the dW GEMM's bf16 operand: (H + 64) * 2
+ *  bytes per kept lattice row, not counted against the 16 GiB chunk budget or the 56 GiB valid_tile_bound rule
+ *  (2.95 GB at B=32 T=512 U=128 H=640, on top of 4.7 GB of numerators). */
 rnntStatus_t rnntb200_joint_workspace_size(const rnntb200JointDesc* desc, size_t* size_bytes);
 
 /** Forward: enc (B,maxT,H), pred (B,maxU,H), W (H,V), bias (V) fp32 device; labels (B,maxU-1),

@@ -9,12 +9,11 @@
 //                   scale, (1 - tanh^2(enc+pred)) (enc / pred rows staged in shared memory by TMA) and the tile's sums
 //                   over u (-> d_enc, accumulated in shared memory along
 //                   a run of tiles and stored once) and over t (-> one fp32 partial plane of d_pred per t-block).
-//                   Neither dl nor dZ ever exists in HBM.
-//   bwd_dw_kernel   [dW; db][H+1,V] (+)= ([rs_row * z, rs_row])^T . E'  as a split-K GEMM over the lattice rows: the A operand
-//                   is REGENERATED from enc/pred (tanh, times the row scale, K-major SWIZZLE_128B) by a producer warpgroup
-//                   into a ring ahead of the two MMA warpgroups, from inputs TMA brought into shared memory a slot ahead;
-//                   row H of A is the row scale itself, so row H of the product is db = sum_rows dl.  The B operand is E'
-//                   loaded MN-major by TMA.  Partial tiles go to fp32 planes (deterministic), summed by sum_planes_kernel.
+//                   Neither dl nor dZ ever exists in HBM.  The epilogue also stores the dW GEMM's A operand
+//                   zs[row, :] = [bf16(rs_row * z), bf16(rs_row)], from the tanh it evaluates anyway.
+//   bwd_dw_kernel   [dW; db][H+1,V] (+)= zs^T . E'  as a split-K GEMM over the lattice rows, both operands MN-major from
+//                   TMA; column H of zs is the row scale itself, so row H of the product is db = sum_rows dl.  Partial
+//                   tiles go to fp32 planes (deterministic), summed by sum_planes_kernel.
 //
 // All operands bf16 (E' needs the exponent range: it is relative to a reference that may lie far below the row maximum),
 // fp32 accumulation.  Tile geometry: 16 x 8 lattice tiles (TT = 16 time steps, UU = 8 label positions), row r = tl*8 + ul;
@@ -30,8 +29,8 @@ constexpr int DZ_NC = 128;              // h columns per dZ pass (m64n128 accumu
 constexpr int DZ_GS_LD = DZ_NC + 8;     // row stride (floats) of the staged gradient tile
 constexpr int DZ_MAX_STAGES = 4;
 constexpr int DZ_IN_ENC = 0, DZ_IN_PRED = 16 * DZ_NC * 4, DZ_IN_BYTES = DZ_IN_PRED + 8 * DZ_NC * 4;   // a pass's enc / pred slice
-constexpr int DW_NV = 128;              // vocabulary columns per dW output tile
-constexpr int DW_STAGES = 4;            // K steps in flight between the producers and the MMA warpgroups (A + B per stage)
+constexpr int DW_NV = 256;              // vocabulary columns per dW CTA tile
+constexpr int DW_STAGES = 4;            // K steps in flight between the TMA lane and the MMA warpgroups (A + B per stage)
 
 struct BwdParams {
     const float* enc; const float* pred;
@@ -46,8 +45,10 @@ struct BwdParams {
     int dz_stages;
     float* d_enc;               // (B, maxT, H), rows of this launch's utterances are fully written
     float* ppred;               // (nTb, nb, maxU, H) partial planes of d_pred
+    __nv_bfloat16* zs;          // (rows of the kept arrays, zs_ld) the dW operand: column h < H rs * z, column H rs
+    int zs_ld;
     // ---- dW kernel
-    int nVT, nHB, S;            // v-tiles, 128-row blocks of [H rows of dW, db], K splits
+    int nVT, nHB, S;            // DW_NV-column v-tiles, 128-row blocks of [H rows of dW, db], K splits
     float* dWp;                 // (S, H, V) partial planes of dW (zeroed by the host, accumulated over utterance chunks)
     float* dbp;                 // (S, V) partial planes of db
 };
@@ -67,6 +68,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                                                                 const __grid_constant__ CUtensorMap tmap_w,
                                                                 const __grid_constant__ CUtensorMap tmap_enc,
                                                                 const __grid_constant__ CUtensorMap tmap_pred,
+                                                                const __grid_constant__ CUtensorMap tmap_zs,
                                                                 const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -88,6 +90,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
     if (warp == 8 && lane == 0) {
         ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_w); ptx::prefetch_tmap(&tmap_enc); ptx::prefetch_tmap(&tmap_pred);
     }
+    if (threadIdx.x == 0) ptx::prefetch_tmap(&tmap_zs);
     for (int i = threadIdx.x; i < 16 * p.H; i += BWD_THREADS) dacc[i] = 0.f;
     __syncthreads();
     const int nruns = p.nb * p.nTb;
@@ -143,8 +146,10 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
             if (tslot < 0) continue;            // as the TMA role: its d_pred partial plane is not written, and not summed
             float rs[2];
 #pragma unroll
-            for (int ri = 0; ri < 2; ++ri)      // 0 outside the lattice and the windows
+            for (int ri = 0; ri < 2; ++ri) {    // 0 outside the lattice and the windows
                 rs[ri] = __ldg(p.rowscale + (size_t)tslot * 128 + Ra + 8 * ri);
+                if (q == 0) p.zs[((size_t)tslot * 128 + Ra + 8 * ri) * p.zs_ld + p.H] = __float2bfloat16_rn(rs[ri]);   // db row
+            }
             for (int pass = 0; pass < NPASS; ++pass) {
                 const int n0 = pass * DZ_NC;
                 float acc[64];
@@ -167,9 +172,14 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                 ptx::wgmma_wait<0>();
                 if (t128 == 0) ptx::mbar_arrive(&empty[prev]);
                 ptx::fence_regs(acc);
-                // ---- g = rs * acc * (1 - tanh^2(enc + pred)) -> staged tile
+                // ---- g = rs * acc * (1 - tanh^2(enc + pred)) -> staged tile, and the dW operand bf16(rs * z) -> zp (0 where
+                //      rs == 0, as g: padding outside the lattice never reaches dW).  The previous pass's operand store must
+                //      have read the staged tile first.
+                if (threadIdx.x == 0) ptx::bulk_wait_group_read<0>();
+                ptx::named_bar_sync(1, 256);
                 ptx::mbar_wait(in_full, iph);
                 iph ^= 1;
+                uint32_t zp[2][16];
 #pragma unroll
                 for (int ri = 0; ri < 2; ++ri) {
                     const int r = Ra + 8 * ri;
@@ -180,11 +190,13 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                     for (int j = 0; j < 16; ++j) {
                         const int h = n0 + 8 * j + 2 * q;
                         float2 g = make_float2(0.f, 0.f);
+                        zp[ri][j] = 0u;
                         if (rs[ri] != 0.f && h < p.H) {
                             const float2 e = ptx::lds64f(erow + 32u * j), pq = ptx::lds64f(prow + 32u * j);
                             const float z0 = ptx::tanh_approx(e.x + pq.x), z1 = ptx::tanh_approx(e.y + pq.y);
                             const float d0 = acc[4 * j + 2 * ri] * rs[ri], d1 = acc[4 * j + 2 * ri + 1] * rs[ri];
                             g = make_float2(fmaf(-d0 * z0, z0, d0), fmaf(-d1 * z1, z1, d1));
+                            zp[ri][j] = ptx::pack_bf16x2(z0 * rs[ri], z1 * rs[ri]);
                         }
                         *reinterpret_cast<float2*>(grow + 8 * j) = g;
                     }
@@ -218,6 +230,24 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
                     *reinterpret_cast<float4*>(p.ppred + (((size_t)tb * p.nb + bl) * p.maxU + u) * p.H + n0 + col) = sum;
                 }
                 ptx::named_bar_sync(1, 256);
+                // ---- the pass's columns of the dW operand: two [128 rows x 64 h] SWIZZLE_128B boxes in the free staged tile,
+                //      stored by TMA (columns past H are clipped by the tensor map)
+                const uint32_t zs_a = ptx::smem_u32(gs);
+#pragma unroll
+                for (int ri = 0; ri < 2; ++ri) {
+                    const int r = Ra + 8 * ri;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j)
+                        ptx::sts32(zs_a + (uint32_t)((j >> 3) * 16384 + r * 128 + (((j & 7) ^ (r & 7)) << 4) + 4 * q), zp[ri][j]);
+                }
+                ptx::fence_proxy_async_smem();
+                ptx::named_bar_sync(1, 256);
+                if (threadIdx.x == 0) {
+                    const uint64_t pol = ptx::l2_policy_evict_first();
+                    ptx::tma_store_2d(&tmap_zs, gs, n0, tslot * 128, pol);
+                    if (n0 + 64 < p.H) ptx::tma_store_2d(&tmap_zs, reinterpret_cast<uint8_t*>(gs) + 16384, n0 + 64, tslot * 128, pol);
+                    ptx::bulk_commit_group();
+                }
             }
         }
         // ---- the run is complete: its d_enc rows leave once (each entry is read and cleared by the thread that stores it)
@@ -227,6 +257,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) bwd_dz_kernel(const __grid_con
             dacc[i] = 0.f;
         }
     }
+    if (threadIdx.x == 0) ptx::bulk_wait_group<0>();      // the dW operand has reached global memory
 }
 
 struct DzGeom { int stages; size_t smem_bytes; bool ok; };
@@ -267,163 +298,91 @@ __global__ void __launch_bounds__(256) sum_pred_planes_kernel(const float4* __re
 // dW kernel
 // ---------------------------------------------------------------------------------------------------------------
 // CTA = (v-tile of DW_NV columns, 128-row block of [dW rows 0..H-1, db], split of the lattice rows).  K step = half a tile
-// (64 lattice rows: 8 time steps x 8 label positions).  Warp-specialised:
-//   warps 0-7    two consumer warpgroups (64 rows of the block each): wait for a stage, 4 x wgmma m64n128k16, release it
-//   warps 8-15   two producer warpgroups: build A [128 h x 64 k] = bf16(rs_row * tanh(enc + pred)) for both consumers from
-//                the slot's inputs in shared memory; thread = one A row, producer warpgroup = 4 of a K step's 8 time rows.
-//                Each SM sub-partition holds two producer warps, so the tanh work uses every MUFU unit and one warp's
-//                shared-memory latency is hidden behind the other's arithmetic (with a single producer warp per
-//                sub-partition the kernel was about 14 % slower at C3).
-//   warp 16      TMA: per slot the enc [16 x 128 h] / pred [8 x 128 h] fp32 boxes, the 128 row scales and the slot's meta
-//                into the input ring one slot ahead; per K step the E' boxes [64 k x 128 v] into the stage ring.
-// A stage holds A and B of one K step; its full barrier completes with the TMA bytes and one arrival per producer warp.
-// A warpgroup whose 64 rows all lie past row H (the second half of the db-only block when H % 128 == 0) does nothing.
-constexpr int DW_PWG = 2;                                   // producer warpgroups
-constexpr int DW_TMA_WARP = 8 + 4 * DW_PWG, DW_THREADS = 32 * (DW_TMA_WARP + 1);
-constexpr int DW_TL = 8 / DW_PWG;                           // time rows of a K step per producer thread
-constexpr int DW_IN_STAGES = 3;
-constexpr int DW_IN_ENC = 0, DW_IN_PRED = 8192, DW_IN_RS = 12288, DW_IN_META = 12800, DW_IN_BYTES = 13312;
+// (64 lattice rows: 8 time steps x 8 label positions).  Both operands come from the workspace by TMA:
+//   A = the dW operand zs (written by bwd_dz_kernel), rows [64 k] x columns [128 h] as two [64 k x 64 h] SWIZZLE_128B boxes,
+//       i.e. MN-major A (one box per consumer warpgroup); columns past H read as zeros, column H is the row scale (db)
+//   B = E' [64 k x DW_NV v] as DW_NV / 64 boxes [64 k x 64 v], MN-major.
+//   warps 0-7    two consumer warpgroups (64 rows of the block each): wait for a stage, 4 x wgmma m64n256k16, release it
+//   warp 8       TMA
+// A warpgroup whose 64 rows all lie past row H (the second half of the db-only block when H % 128 == 0) does nothing, and
+// its A box is not loaded.  A last v-tile narrower than DW_NV leaves its missing B boxes as zeros: their columns are
+// computed as zeros and not stored.
+// Each dW / db element is the same chain of k16 products over the same lattice rows, in the same order and on the same
+// operand values, whatever DW_NV is: the split plan below is that of 128-column v-tiles (dw_geometry).
+constexpr int DW_THREADS = 288;
+constexpr int DW_NB = DW_NV / 64;                           // B boxes per stage
+constexpr int DW_STAGE_BYTES = 16384 + DW_NB * 8192;        // A [64 k x 128 h] + B [64 k x DW_NV v]
 struct DwWork { int vt, hb, split; };
+// split-major: the CTAs resident at once cover every (v-tile, h-block) pair of a few splits, so each zs and E' row block
+// is fetched from HBM about once and read by the others from L2
 __device__ __forceinline__ DwWork dw_decode(const BwdParams& p, int cta) {
     DwWork w;
-    const int per_vt = p.nHB * p.S;
-    w.vt = cta / per_vt;
-    const int rem = cta - w.vt * per_vt;
-    w.hb = rem / p.S;
-    w.split = rem - w.hb * p.S;
+    w.hb = cta % p.nHB;
+    const int rem = cta / p.nHB;
+    w.vt = rem % p.nVT;
+    w.split = rem / p.nVT;
     return w;
 }
 
 __global__ void __launch_bounds__(DW_THREADS, 1) bwd_dw_kernel(const __grid_constant__ CUtensorMap tmap_e,
-                                                               const __grid_constant__ CUtensorMap tmap_enc,
-                                                               const __grid_constant__ CUtensorMap tmap_pred, const BwdParams p) {
+                                                               const __grid_constant__ CUtensorMap tmap_zs, const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    // stage st: B = E' [64 k x 128 v] as two [64 k x 64 v] boxes (MN-major, SW128) at bsm + st * 16384 | A [128 h x 64 k]
-    // K-major SW128 at asm_ + st * 16384 (rows 0-63: consumer 0, rows 64-127: consumer 1) | input ring | barriers
-    uint8_t* bsm = smem;
-    uint8_t* asm_ = smem + DW_STAGES * 16384;
-    uint8_t* ism = asm_ + DW_STAGES * 16384;
-    uint64_t* full = reinterpret_cast<uint64_t*>(ism + DW_IN_STAGES * DW_IN_BYTES);
+    // stage st at smem + st * DW_STAGE_BYTES: A boxes (h 0-63 | h 64-127 of the block) at +0 / +8192, B box j at 16384 + j * 8192
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + DW_STAGES * DW_STAGE_BYTES);
     uint64_t* empty = full + DW_STAGES;
-    uint64_t* in_full = empty + DW_STAGES;
-    uint64_t* in_empty = in_full + DW_IN_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const DwWork wk = dw_decode(p, blockIdx.x);
     const int v0 = wk.vt * DW_NV, nbox = min(DW_NV, p.V - v0) >> 6, h0 = wk.hb * 128;
     const int nwg = h0 + 64 > p.H ? 1 : 2;                             // consumer warpgroups with a row <= H
     if (threadIdx.x == 0) {
-        for (int i = 0; i < DW_STAGES; ++i) { ptx::mbar_init(&full[i], 1 + 2 * DW_PWG * nwg); ptx::mbar_init(&empty[i], nwg); }
-        for (int i = 0; i < DW_IN_STAGES; ++i) { ptx::mbar_init(&in_full[i], 1); ptx::mbar_init(&in_empty[i], 2 * DW_PWG * nwg); }
+        for (int i = 0; i < DW_STAGES; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], nwg); }
         ptx::fence_barrier_init();
     }
-    if (nbox == 1)      // a 64-wide last v-tile: the second box of every stage is never loaded and reads as zeros
-        for (int i = threadIdx.x; i < DW_STAGES * 512; i += DW_THREADS)
-            reinterpret_cast<uint4*>(bsm + (size_t)(i >> 9) * 16384 + 8192)[i & 511] = make_uint4(0u, 0u, 0u, 0u);
+    if (nbox < DW_NB)   // a narrower last v-tile: the B boxes past it are never loaded and read as zeros
+        for (int i = threadIdx.x; i < DW_STAGES * (DW_NB - nbox) * 512; i += DW_THREADS) {
+            const int per = (DW_NB - nbox) * 512, st = i / per, k = i - st * per;
+            reinterpret_cast<uint4*>(smem + (size_t)st * DW_STAGE_BYTES + 16384 + nbox * 8192)[k] = make_uint4(0u, 0u, 0u, 0u);
+        }
     ptx::fence_proxy_async_smem();
-    if (warp == DW_TMA_WARP && lane == 0) { ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_enc); ptx::prefetch_tmap(&tmap_pred); }
+    if (warp == 8 && lane == 0) { ptx::prefetch_tmap(&tmap_e); ptx::prefetch_tmap(&tmap_zs); }
     __syncthreads();
     const long long cnt = *p.count;
     const int s_beg = (int)(cnt * wk.split / p.S), s_end = (int)(cnt * (wk.split + 1) / p.S);
 
-    if (warp == DW_TMA_WARP) {
-        // ===================== TMA: the producer's inputs per slot, B = kept numerators per K step =====================
+    if (warp == 8) {
+        // ===================== TMA: per K step the zs boxes and the E' boxes =====================
         if (lane == 0) {
-            int st = 0, is = 0; uint32_t ph = 0, iph = 0;
-            auto load_inputs = [&](int s) {
-                ptx::mbar_wait(&in_empty[is], iph ^ 1);
-                uint8_t* in = ism + (size_t)is * DW_IN_BYTES;
-                const int4 m = __ldg(p.slot_meta + s);
-                ptx::sts128(ptx::smem_u32(in + DW_IN_META), make_uint4((uint32_t)m.x, (uint32_t)m.y, (uint32_t)m.z, (uint32_t)m.w));
-                ptx::mbar_arrive_expect_tx(&in_full[is], (uint32_t)(DW_IN_META - DW_IN_ENC));
-                ptx::tma_load_2d(in + DW_IN_ENC, &tmap_enc, &in_full[is], h0, m.x);
-                ptx::tma_load_2d(in + DW_IN_PRED, &tmap_pred, &in_full[is], h0, m.y);
-                ptx::bulk_load_1d(in + DW_IN_RS, p.rowscale + (size_t)s * 128, 512u, &in_full[is]);
-                if (++is == DW_IN_STAGES) { is = 0; iph ^= 1; }
-            };
-            if (s_beg < s_end) load_inputs(s_beg);
-            for (int s = s_beg; s < s_end; ++s) {
-                if (s + 1 < s_end) load_inputs(s + 1);
-                for (int half = 0; half < 2; ++half) {
-                    ptx::mbar_wait(&empty[st], ph ^ 1);
-                    ptx::mbar_arrive_expect_tx(&full[st], (uint32_t)nbox * 8192u);
-                    for (int j = 0; j < nbox; ++j)
-                        ptx::tma_load_2d(bsm + (size_t)st * 16384 + j * 8192, &tmap_e, &full[st], v0 + 64 * j, s * 128 + half * 64);
-                    if (++st == DW_STAGES) { st = 0; ph ^= 1; }
-                }
-            }
-        }
-        return;
-    }
-
-    if (warp >= 8) {
-        // ===================== producers: A row `row`, time rows [tl0, tl0 + DW_TL) of every K step =====================
-        const int row = (threadIdx.x - 256) & 127, tl0 = ((threadIdx.x - 256) >> 7) * DW_TL, h = h0 + row;
-        if (h0 + (row >> 6) * 64 > p.H) return;                        // rows of an idle consumer warpgroup
-        const int kind = h < p.H ? 0 : (h == p.H ? 1 : 2);              // z row | row-scale row (db) | zero row
-        const uint32_t a_a = ptx::smem_u32(asm_) + (uint32_t)row * 128u, i_a = ptx::smem_u32(ism);
-        int st = 0, is = 0; uint32_t ph = 0, iph = 0;
-        for (int s = s_beg; s < s_end; ++s) {
-            ptx::mbar_wait_warp(&in_full[is], iph);
-            const uint32_t in = i_a + (uint32_t)is * DW_IN_BYTES;
-            // 8 pred rows and 16 enc rows of column h; rows past the padded arrays are clamped (their row scale is 0)
-            const uint4 m = ptx::lds128(in + DW_IN_META);
-            float pv[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) pv[k] = __uint_as_float(ptx::lds32(in + DW_IN_PRED + (uint32_t)(min(k, (int)m.w - 1) * 128 + row) * 4u));
-            for (int half = 0; half < 2; ++half) {
-                // every shared load of the half is issued before the first tanh: the accesses are volatile, so they keep
-                // source order, and with one or two producer warps per sub-partition nothing else hides their latency
-                float ev[DW_TL];
-                float4 rs4[2 * DW_TL];
-#pragma unroll
-                for (int j = 0; j < DW_TL; ++j)
-                    ev[j] = __uint_as_float(ptx::lds32(in + DW_IN_ENC + (uint32_t)(min(half * 8 + tl0 + j, (int)m.z - 1) * 128 + row) * 4u));
-#pragma unroll
-                for (int j = 0; j < 2 * DW_TL; ++j) rs4[j] = ptx::lds128f(in + DW_IN_RS + (uint32_t)(half * 64 + tl0 * 8 + 4 * j) * 4u);
-                ptx::mbar_wait_warp(&empty[st], ph ^ 1);
-                const uint32_t abuf = a_a + (uint32_t)st * 16384u;
-#pragma unroll
-                for (int j = 0; j < DW_TL; ++j) {
-                    const int tl = tl0 + j;
-                    const float rsv[8] = {rs4[2 * j].x, rs4[2 * j].y, rs4[2 * j].z, rs4[2 * j].w,
-                                          rs4[2 * j + 1].x, rs4[2 * j + 1].y, rs4[2 * j + 1].z, rs4[2 * j + 1].w};
-                    float z[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        z[k] = kind == 0 ? ptx::tanh_approx(ev[j] + pv[k]) * rsv[k] : (kind == 1 ? rsv[k] : 0.f);
-                    ptx::sts128(abuf + (uint32_t)((tl ^ (row & 7)) << 4),
-                                make_uint4(ptx::pack_bf16x2(z[0], z[1]), ptx::pack_bf16x2(z[2], z[3]), ptx::pack_bf16x2(z[4], z[5]),
-                                           ptx::pack_bf16x2(z[6], z[7])));
-                }
-                ptx::fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&full[st]);
+            int st = 0; uint32_t ph = 0;
+            for (int step = 2 * s_beg; step < 2 * s_end; ++step) {
+                ptx::mbar_wait(&empty[st], ph ^ 1);
+                ptx::mbar_arrive_expect_tx(&full[st], (uint32_t)(nwg + nbox) * 8192u);
+                uint8_t* sb = smem + (size_t)st * DW_STAGE_BYTES;
+                for (int w = 0; w < nwg; ++w) ptx::tma_load_2d(sb + w * 8192, &tmap_zs, &full[st], h0 + 64 * w, step * 64);
+                for (int j = 0; j < nbox; ++j) ptx::tma_load_2d(sb + 16384 + j * 8192, &tmap_e, &full[st], v0 + 64 * j, step * 64);
                 if (++st == DW_STAGES) { st = 0; ph ^= 1; }
             }
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&in_empty[is]);
-            if (++is == DW_IN_STAGES) { is = 0; iph ^= 1; }
         }
         return;
     }
 
-    // ===================== consumer warpgroups: D[64 h x 128 v] += A[64 h x 64 k] . E'[64 k x 128 v] =====================
+    // ===================== consumer warpgroups: D[64 h x DW_NV v] += A[64 h x 64 k] . E'[64 k x DW_NV v] =====================
     const int wg = warp >> 2, t128 = threadIdx.x & 127, q = lane & 3;
     if (h0 + wg * 64 > p.H) return;
-    const uint32_t a_a = ptx::smem_u32(asm_) + (uint32_t)wg * 8192u, b_a = ptx::smem_u32(bsm);
-    float acc[64];
+    const uint32_t s_a = ptx::smem_u32(smem);
+    float acc[DW_NV / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < DW_NV / 2; ++i) acc[i] = 0.f;
     int st = 0, prev = -1; uint32_t ph = 0;
     for (int step = 2 * s_beg; step < 2 * s_end; ++step) {
         ptx::mbar_wait_warp(&full[st], ph);
-        const uint64_t ad = ptx::gmma_desc_k_sw128(a_a + (uint32_t)st * 16384u), bd = ptx::gmma_desc_mn_sw128(b_a + (uint32_t)st * 16384u, 8192u);
+        const uint32_t sa = s_a + (uint32_t)st * DW_STAGE_BYTES;
+        const uint64_t ad = ptx::gmma_desc_mn_sw128(sa + (uint32_t)wg * 8192u, 8192u), bd = ptx::gmma_desc_mn_sw128(sa + 16384u, 8192u);
         ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)   // K = 16 lattice rows per MMA: 32 B along A's rows, 16 x 128 B of B
-            ptx::wgmma_m64n128_bf16<1>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 128), 1u);
+        for (int k = 0; k < 4; ++k)   // K = 16 lattice rows per MMA: 16 x 128 B of A and of every B box
+            ptx::wgmma_m64n256_bf16<1, 1>(acc, ad + (uint64_t)(k * 128), bd + (uint64_t)(k * 128), 1u);
         ptx::wgmma_commit();
         ptx::wgmma_wait<1>();        // the previous step's MMAs have retired: its stage is free
         if (prev >= 0 && t128 == 0) ptx::mbar_arrive(&empty[prev]);
@@ -434,7 +393,7 @@ __global__ void __launch_bounds__(DW_THREADS, 1) bwd_dw_kernel(const __grid_cons
     if (prev >= 0 && t128 == 0) ptx::mbar_arrive(&empty[prev]);
     ptx::fence_regs(acc);
     if (s_end <= s_beg) return;
-    // ---- epilogue: rows (Ra, Ra + 8) x 32 columns of the block -> accumulated into the split's partial plane
+    // ---- epilogue: rows (Ra, Ra + 8) x DW_NV / 4 columns of the block -> accumulated into the split's partial plane
     const int Ra = h0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
     for (int ri = 0; ri < 2; ++ri) {
@@ -442,7 +401,7 @@ __global__ void __launch_bounds__(DW_THREADS, 1) bwd_dw_kernel(const __grid_cons
         if (hr > p.H) continue;
         float* dst = hr < p.H ? p.dWp + ((size_t)wk.split * p.H + hr) * p.V : p.dbp + (size_t)wk.split * p.V;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < DW_NV / 8; ++j) {
             const int v = v0 + 8 * j + 2 * q;
             if (v >= p.V) continue;
             float2* d2 = reinterpret_cast<float2*>(dst + v);
@@ -452,18 +411,20 @@ __global__ void __launch_bounds__(DW_THREADS, 1) bwd_dw_kernel(const __grid_cons
     }
 }
 
-struct DwGeom { int nVT, nHB, S; size_t smem_bytes; };
-// S: lattice-row splits for about four waves of CTAs.  Besides balancing the grid this bounds the length of each fp32
-// accumulation chain (db[blank] is a same-sign sum over every lattice row: at C3 one split per SM would chain 1 M rows).
-// A pure function of (H, V), as the workspace holds S planes.
+struct DwGeom { int nVT, nHB, S, nCT; size_t smem_bytes; };
+// S: lattice-row splits for about four waves of 128-column CTAs.  Besides balancing the grid this bounds the length of
+// each fp32 accumulation chain (db[blank] is a same-sign sum over every lattice row: at C3 one split per SM would chain
+// 1 M rows).  A pure function of (H, V), as the workspace holds S planes; it stays that of 128-column v-tiles (nVT) so
+// that the split boundaries, and with them dW's bits, do not depend on the CTA tile width (nCT v-tiles of DW_NV).
 inline DwGeom dw_geometry(int H, int V) {
     DwGeom g{};
-    g.nVT = (V + DW_NV - 1) / DW_NV;
+    g.nVT = (V + 127) / 128;
+    g.nCT = (V + DW_NV - 1) / DW_NV;
     g.nHB = H / 128 + 1;                    // rows 0 .. H (row H: db)
     g.S = 4 * TC_SMS / (g.nVT * g.nHB);
     if (g.S < 1) g.S = 1;
     if (g.S > 64) g.S = 64;
-    g.smem_bytes = 1024 + (size_t)DW_STAGES * 32768 + (size_t)DW_IN_STAGES * DW_IN_BYTES + 2 * (DW_STAGES + DW_IN_STAGES) * 8;
+    g.smem_bytes = 1024 + (size_t)DW_STAGES * DW_STAGE_BYTES + 2 * DW_STAGES * 8;
     return g;
 }
 

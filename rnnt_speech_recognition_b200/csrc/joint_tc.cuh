@@ -204,13 +204,14 @@ inline PFN_encodeTiled get_encode_fn() {
     }
     return fn;
 }
-// 2-D row-major bf16 matrix [rows x cols] (cols contiguous), box [box_rows x 64 cols], SWIZZLE_128B
+// 2-D row-major bf16 matrix [rows x cols] (cols contiguous, rows `ld` elements apart: cols when 0), box [box_rows x 64
+// cols], SWIZZLE_128B
 inline bool make_tmap_bf16(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                           uint32_t box_cols = 64) {
+                           uint32_t box_cols = 64, uint64_t ld = 0) {
     PFN_encodeTiled fn = get_encode_fn();
     if (!fn) return false;
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 2};
+    cuuint64_t strides[1] = {(ld ? ld : cols) * 2};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     return fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
@@ -244,6 +245,8 @@ struct TcScratch {
     float* dWp;                             // (S_max, H, V) fp32 split-K planes of dW (bwd_dw_kernel)
     float* dbp;                             // (S_max, V) planes of db
     float* rowscale;                        // (rows_chunk) per-row scale of the logit gradients (row_scale_kernel)
+    __nv_bfloat16* zs;                      // (rows_chunk, zs_ld) bf16 dW operand [rs * z, rs] (bwd_dz_kernel)
+    int zs_ld;                              // H + 64: rows start on 128-byte lines
     int bchunk;                             // utterances per chunk
     size_t rows_chunk;                      // bchunk * tiles_per_utt * 128
     size_t bytes;
@@ -321,6 +324,12 @@ inline TcScratch tc_scratch_layout(const rnntb200JointDesc& d, void* base) {
     s.dWp = reinterpret_cast<float*>(take((size_t)wg.S * d.H * d.V * 4));
     s.dbp = reinterpret_cast<float*>(take((size_t)wg.S * d.V * 4));
     s.rowscale = reinterpret_cast<float*>(take(s.rows_chunk * 4));
+    // the dW operand is not part of the chunk plan above: the plan (and with it how many times the dW planes are
+    // accumulated) sizes the kept numerators alone, and zs adds rows_chunk * (H + 64) * 2 bytes on top of it.  Rows
+    // start on 128-byte lines, so that every 64-column box row the dZ kernel stores and the dW kernel loads is one whole
+    // line (with a row stride of H + 8, merely 16-byte aligned, the C3 step was 2 ms slower).
+    s.zs_ld = d.H + 64;
+    s.zs = reinterpret_cast<__nv_bfloat16*>(take(s.rows_chunk * s.zs_ld * 2));
     s.bytes = (size_t)(p - static_cast<char*>(base));
     return s;
 }
@@ -426,9 +435,13 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
     if (cudaMemsetAsync(sc.dWp, 0, sizeof(float) * (size_t)wg.S * d.H * d.V, s) != cudaSuccess ||
         cudaMemsetAsync(sc.dbp, 0, sizeof(float) * (size_t)wg.S * d.V, s) != cudaSuccess)
         return RNNT_STATUS_MEMOPS_FAILED;
-    CUtensorMap tm_e128, tm_e64, tm_w, tm_enc, tm_pred;
+    // the dW operand is stored through a map H columns wide (column H, the row scale, is written directly) and loaded
+    // through one H + 1 wide, so that the columns past H of the last row block read as zeros
+    CUtensorMap tm_e128, tm_e64, tm_w, tm_enc, tm_pred, tm_zs_st, tm_zs_ld;
     if (!make_tmap_bf16(&tm_e128, sc.dl, sc.rows_chunk, d.V, 128) || !make_tmap_bf16(&tm_e64, sc.dl, sc.rows_chunk, d.V, 64) ||
         !make_tmap_bf16(&tm_w, sc.Wb, d.H, d.V, DZ_NC) ||
+        !make_tmap_bf16(&tm_zs_st, sc.zs, sc.rows_chunk, d.H, 128, 64, sc.zs_ld) ||
+        !make_tmap_bf16(&tm_zs_ld, sc.zs, sc.rows_chunk, d.H + 1, 64, 64, sc.zs_ld) ||
         !make_tmap_f32(&tm_enc, enc, (uint64_t)d.B * d.maxT, d.H, BW_TT) || !make_tmap_f32(&tm_pred, pred, (uint64_t)d.B * d.maxU, d.H, BW_UU)) {
         fprintf(stderr, "rnnt_b200: cuTensorMapEncodeTiled failed\n");
         return RNNT_STATUS_EXECUTION_FAILED;
@@ -453,8 +466,8 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         p.maxT = d.maxT; p.maxU = d.maxU; p.H = d.H; p.V = d.V;
         p.nTb = g.nTb; p.nUb = g.nUb; p.b0 = b0; p.nb = nb;
         p.slot = sc.slot; p.slot_meta = sc.slot_meta; p.count = sc.count; p.rowscale = sc.rowscale;
-        p.dz_stages = zg.stages; p.d_enc = d_enc; p.ppred = sc.ppl;
-        p.nVT = wg.nVT; p.nHB = wg.nHB; p.S = wg.S; p.dWp = sc.dWp; p.dbp = sc.dbp;
+        p.dz_stages = zg.stages; p.d_enc = d_enc; p.ppred = sc.ppl; p.zs = sc.zs; p.zs_ld = sc.zs_ld;
+        p.nVT = wg.nCT; p.nHB = wg.nHB; p.S = wg.S; p.dWp = sc.dWp; p.dbp = sc.dbp;
         // rows of d_enc whose t-block lies outside the utterance are never visited by the dZ kernel (a t-block inside it
         // without a valid tile is: its rows are stored as the zeros they are)
         if (cudaMemsetAsync(d_enc + (size_t)b0 * d.maxT * d.H, 0, sizeof(float) * (size_t)nb * d.maxT * d.H, s) != cudaSuccess)
@@ -462,7 +475,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         {
             const int nruns = nb * g.nTb;
             ScopedTimer tmr("bwd_dz_kernel", s);
-            bwd_dz_kernel<<<nruns < sms ? nruns : sms, BWD_THREADS, zg.smem_bytes, s>>>(tm_e128, tm_w, tm_enc, tm_pred, p);
+            bwd_dz_kernel<<<nruns < sms ? nruns : sms, BWD_THREADS, zg.smem_bytes, s>>>(tm_e128, tm_w, tm_enc, tm_pred, tm_zs_st, p);
         }
         {
             const size_t n4 = (size_t)nb * d.maxU * d.H / 4;
@@ -473,7 +486,7 @@ inline rnntStatus_t tc_backward(const rnntb200JointDesc& d, void* scratch, const
         }
         {
             ScopedTimer tmr("bwd_dw_kernel", s);
-            bwd_dw_kernel<<<wg.nVT * wg.nHB * wg.S, DW_THREADS, wg.smem_bytes, s>>>(tm_e64, tm_enc, tm_pred, p);
+            bwd_dw_kernel<<<wg.nCT * wg.nHB * wg.S, DW_THREADS, wg.smem_bytes, s>>>(tm_e64, tm_zs_ld, p);
         }
         *launches += 3;
         if (cudaGetLastError() != cudaSuccess) return RNNT_STATUS_EXECUTION_FAILED;
